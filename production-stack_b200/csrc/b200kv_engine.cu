@@ -267,72 +267,12 @@ int env_int(const char* name, int dflt) {
   return (v && *v) ? std::atoi(v) : dflt;
 }
 
-// ---- run construction (host) -----------------------------------------------------------------
-// slot_mapping[i] for op-relative token i (vllm_v1_adapter.py:368-375).  A run never crosses a
-// vLLM block or a chunk boundary, so both sides of every run are contiguous byte ranges.
-// For HND tiles a run additionally stops at every chunk-side tile boundary, and runs are split
-// into `full` (one whole aligned block on both sides: a contiguous tile, moved by the bulk kernel
-// exactly like NHD) and `partial` (moved per head by kv_hnd_partial_kernel).  NHD: all `full`.
-struct RunSink {
-  std::vector<Run>* full;
-  std::vector<Run>* partial;
-  bool hnd;
-  int32_t bs;
-  bool both_paged;  // peer pull: `b` is a paged slot too
-  void push(const Run& r) const {
-    if (!hnd || !partial) { full->push_back(r); return; }  // FP8 kernels take one sorted list
-    const bool whole = r.n == bs && (r.a % bs) == 0 && (r.b % bs) == 0;
-    (whole ? full : partial)->push_back(r);
-  }
-};
-
-int build_runs(const b200kv_ctx* ctx, const int64_t* slots, int64_t tok_begin, int64_t tok_end,
-               int64_t b_shift, std::vector<Run>* full, std::vector<Run>* partial) {
+// ---- run construction (host): b200kv_runs.h --------------------------------------------------
+int op_runs(const b200kv_ctx* ctx, const int64_t* slots, int64_t tok_begin, int64_t tok_end, int64_t b_shift,
+            std::vector<Run>* full, std::vector<Run>* partial) {
   const Geometry& g = ctx->g;
-  const RunSink sink{full, partial, g.hnd, static_cast<int32_t>(g.bs), false};
-  const int64_t max_slot = static_cast<int64_t>(ctx->cfg.n_blocks) * g.bs;
-  Run cur{0, 0, 0};
-  for (int64_t i = tok_begin; i < tok_end; ++i) {
-    const int64_t s = slots[i];
-    if (s < 0 || s >= max_slot) return B200KV_EINVAL;
-    const bool extend = cur.n > 0 && s == static_cast<int64_t>(cur.a) + cur.n && (s % g.bs) != 0 &&
-                        ((i - b_shift) % g.C) != 0 && !(g.hnd && ((i - b_shift) % g.bs) == 0);
-    if (extend) {
-      ++cur.n;
-    } else {
-      if (cur.n) sink.push(cur);
-      cur.a = static_cast<int32_t>(s);
-      cur.b = static_cast<int32_t>(i - b_shift);
-      cur.n = 1;
-    }
-  }
-  if (cur.n) sink.push(cur);
-  return B200KV_OK;
-}
-
-int build_pull_runs(const b200kv_ctx* ctx, const Peer& peer, const int64_t* src, const int64_t* dst,
-                    int64_t n, std::vector<Run>* full, std::vector<Run>* partial) {
-  const Geometry& g = ctx->g;
-  const RunSink sink{full, partial, g.hnd, static_cast<int32_t>(g.bs), true};
-  const int64_t max_dst = static_cast<int64_t>(ctx->cfg.n_blocks) * g.bs;
-  const int64_t max_src = static_cast<int64_t>(peer.n_blocks) * g.bs;
-  Run cur{0, 0, 0};
-  for (int64_t i = 0; i < n; ++i) {
-    const int64_t s = src[i], d = dst[i];
-    if (s < 0 || s >= max_src || d < 0 || d >= max_dst) return B200KV_EINVAL;
-    const bool extend = cur.n > 0 && s == static_cast<int64_t>(cur.a) + cur.n &&
-                        d == static_cast<int64_t>(cur.b) + cur.n && (s % g.bs) != 0 && (d % g.bs) != 0;
-    if (extend) {
-      ++cur.n;
-    } else {
-      if (cur.n) sink.push(cur);
-      cur.a = static_cast<int32_t>(s);
-      cur.b = static_cast<int32_t>(d);
-      cur.n = 1;
-    }
-  }
-  if (cur.n) sink.push(cur);
-  return B200KV_OK;
+  return build_runs(slots, tok_begin, tok_end, b_shift, static_cast<int64_t>(ctx->cfg.n_blocks) * g.bs,
+                    static_cast<int32_t>(g.bs), static_cast<int32_t>(g.C), g.hnd, full, partial);
 }
 
 // ---- table ring ------------------------------------------------------------------------------
@@ -1127,7 +1067,7 @@ static int gather_scatter(b200kv_ctx* ctx, const int64_t* slots, int64_t n_token
 
   std::vector<Run> runs, partial;
   const bool fp8 = ctx->cfg.format != B200KV_FMT_RAW;   // one sorted run list for every transformed format
-  int rc = build_runs(ctx, slots, 0, n_tokens, 0, &runs, fp8 ? nullptr : &partial);
+  int rc = op_runs(ctx, slots, 0, n_tokens, 0, &runs, fp8 ? nullptr : &partial);
   if (rc) return rc;
   const size_t n_full = runs.size(), n_part = partial.size();
   runs.insert(runs.end(), partial.begin(), partial.end());
@@ -1304,8 +1244,8 @@ static int store_impl(b200kv_ctx* ctx, const uint64_t* keys, const int32_t* chun
       offs[i] = static_cast<uint32_t>(runs.size());
       const int64_t tb = static_cast<int64_t>(t.c) * g.C;
       // dense op-relative token index: chunk i of this batch starts at i*C
-      int rc = build_runs(ctx, slot_mapping, tb, tb + t.n_tok, tb - static_cast<int64_t>(i) * g.C, &runs,
-                          ctx->cfg.format != B200KV_FMT_RAW ? nullptr : &partial);
+      int rc = op_runs(ctx, slot_mapping, tb, tb + t.n_tok, tb - static_cast<int64_t>(i) * g.C, &runs,
+                       ctx->cfg.format != B200KV_FMT_RAW ? nullptr : &partial);
       if (rc) return rc;
       sidx[i] = ctx->store_next;
       ctx->store_next = (ctx->store_next + 1) % static_cast<uint32_t>(n_stage);
@@ -1466,8 +1406,8 @@ static int load_impl(b200kv_ctx* ctx, const uint64_t* keys, const int32_t* chunk
       offs[i] = static_cast<uint32_t>(runs.size());
       const int64_t tb = static_cast<int64_t>(t.c) * g.C;
       std::vector<Run> cf, cp;
-      int rc = build_runs(ctx, slot_mapping, tb, tb + t.n_tok, tb - static_cast<int64_t>(i) * g.C, &cf,
-                          ctx->cfg.format != B200KV_FMT_RAW ? nullptr : &cp);
+      int rc = op_runs(ctx, slot_mapping, tb, tb + t.n_tok, tb - static_cast<int64_t>(i) * g.C, &cf,
+                       ctx->cfg.format != B200KV_FMT_RAW ? nullptr : &cp);
       if (rc) return rc;
       n_full_of[i] = static_cast<uint32_t>(cf.size());
       runs.insert(runs.end(), cf.begin(), cf.end());
@@ -1539,8 +1479,8 @@ static int load_impl(b200kv_ctx* ctx, const uint64_t* keys, const int32_t* chunk
       offs[i] = static_cast<uint32_t>(runs.size());
       const int64_t tb = static_cast<int64_t>(t.c) * g.C;
       std::vector<Run> cf, cp;  // per chunk: whole tiles first, then HND partial-tile runs
-      int rc = build_runs(ctx, slot_mapping, tb, tb + t.n_tok, tb - static_cast<int64_t>(i) * g.C, &cf,
-                          ctx->cfg.format != B200KV_FMT_RAW ? nullptr : &cp);
+      int rc = op_runs(ctx, slot_mapping, tb, tb + t.n_tok, tb - static_cast<int64_t>(i) * g.C, &cf,
+                       ctx->cfg.format != B200KV_FMT_RAW ? nullptr : &cp);
       if (rc) return rc;
       n_full_of[i] = static_cast<uint32_t>(cf.size());
       runs.insert(runs.end(), cf.begin(), cf.end());
@@ -1851,7 +1791,9 @@ extern "C" int b200kv_peer_pull_async(b200kv_ctx* ctx, int32_t peer_id, const in
   *ticket = 0;
 
   std::vector<Run> runs, partial;
-  int rc = build_pull_runs(ctx, peer, src_slots, dst_slots, n_tokens, &runs, &partial);
+  int rc = build_pull_runs(src_slots, dst_slots, n_tokens, static_cast<int64_t>(peer.n_blocks) * ctx->g.bs,
+                           static_cast<int64_t>(ctx->cfg.n_blocks) * ctx->g.bs, static_cast<int32_t>(ctx->g.bs),
+                           ctx->g.hnd, &runs, &partial);
   if (rc) return rc;
   const size_t n_full = runs.size(), n_part = partial.size();
   runs.insert(runs.end(), partial.begin(), partial.end());

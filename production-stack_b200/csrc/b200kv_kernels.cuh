@@ -29,16 +29,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-namespace b200kv {
+#include "b200kv_runs.h"
 
-// One run = consecutive tokens that stay inside one vLLM block and one chunk.
-//   store / load : a = paged slot (block*bs + off) ; b = op-relative token index
-//   peer pull    : a = peer slot                   ; b = local slot
-struct Run {
-  int32_t a;
-  int32_t b;
-  int32_t n;
-};
+namespace b200kv {
 
 struct PagedSide {
   const uint64_t* bases;  // device array [2*L]: K plane of layer l at [2l], V plane at [2l+1]

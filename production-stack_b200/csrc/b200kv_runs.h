@@ -1,0 +1,110 @@
+// b200kv_runs.h — run tables of the copy kernels, built on the host.
+//
+// Host-only (no CUDA header): the engine includes it through b200kv_kernels.cuh, and plain g++
+// compiles it for the equivalence test (tests/test_run_tables.py).
+//
+// A run is a stretch of consecutive tokens that the kernels move as one contiguous byte range on
+// each side.  The builders read the map once: at a run's first token they range-check its slot and
+// compute the run's limit, then extend the run while the slots stay consecutive.  The limit keeps
+// a run's slots below the bound its first slot was checked against, so checking the first slot of
+// each run checks every slot of the map.
+#pragma once
+
+#include <stdint.h>
+
+#include <algorithm>
+#include <vector>
+
+#include "b200kv.h"
+
+namespace b200kv {
+
+// One run = consecutive tokens that stay inside one vLLM block and one chunk.
+//   store / load : a = paged slot (block*bs + off) ; b = op-relative token index
+//   peer pull    : a = peer slot                   ; b = local slot
+struct Run {
+  int32_t a;
+  int32_t b;
+  int32_t n;
+};
+
+// true if slot s lies outside [0, bound)
+inline bool out_of_range(int64_t s, int64_t bound) {
+  return static_cast<uint64_t>(s) >= static_cast<uint64_t>(bound);
+}
+
+// length of the run of p[0, lim) that continues p[0] == s as s, s+1, s+2, ... (lim >= 1).  A whole
+// block of a block table is the common case: it is recognised with one branch-free pass of subtracts
+// and ORs over the window (which vectorises) before the scalar scan that finds where a run ends.
+inline int64_t consecutive(const int64_t* p, int64_t s, int64_t lim) {
+  if (lim == 1 || p[1] != s + 1) return 1;
+  uint64_t diff = 0;
+  for (int64_t k = 2; k < lim; ++k) diff |= static_cast<uint64_t>(p[k]) - static_cast<uint64_t>(s) - k;
+  if (diff == 0) return lim;
+  int64_t n = 2;
+  while (p[n] == s + n) ++n;   // ends before lim: some slot of the window differs
+  return n;
+}
+
+// tokens from x up to (excluding) the next multiple of m above x
+inline int64_t tokens_to_boundary(int64_t x, int64_t m) {
+  const int64_t r = x % m;
+  return r < 0 ? -r : m - r;
+}
+
+// HND tiles: `full` takes runs that are one whole aligned block on both sides (a contiguous tile,
+// moved by the bulk kernel exactly like NHD), `partial` the rest (moved per head by
+// kv_hnd_partial_kernel).  NHD, or no `partial` list (the FP8 / Q4 kernels take one sorted list):
+// everything goes to `full`.
+inline void push_run(const Run& r, int32_t bs, bool hnd, std::vector<Run>* full, std::vector<Run>* partial) {
+  if (!hnd || !partial) { full->push_back(r); return; }
+  const bool whole = r.n == bs && (r.a % bs) == 0 && (r.b % bs) == 0;
+  (whole ? full : partial)->push_back(r);
+}
+
+// Runs of slots[tok_begin, tok_end) (vllm_v1_adapter.py:368-375) for a store / load.  Token i has
+// op-relative index i - b_shift.  A run never crosses a vLLM block on the slot side or a chunk (C
+// tokens) on the op side; for HND it also stops at every op-side tile (bs tokens) boundary.  Returns
+// B200KV_EINVAL if a slot lies outside [0, max_slot); the lists then hold an unspecified prefix.
+inline int build_runs(const int64_t* slots, int64_t tok_begin, int64_t tok_end, int64_t b_shift, int64_t max_slot,
+                      int32_t bs, int32_t C, bool hnd, std::vector<Run>* full, std::vector<Run>* partial) {
+  // room left in the current chunk and tile on the op side; a run ends at or before both, so
+  // subtracting its length and wrapping at zero keeps them exact
+  int64_t chunk_room = tokens_to_boundary(tok_begin - b_shift, C);
+  int64_t tile_room = tokens_to_boundary(tok_begin - b_shift, bs);
+  for (int64_t i = tok_begin; i < tok_end;) {
+    const int64_t s = slots[i];
+    if (out_of_range(s, max_slot)) return B200KV_EINVAL;
+    int64_t lim = std::min({static_cast<int64_t>(bs) - s % bs, max_slot - s, chunk_room, tok_end - i});
+    if (hnd) lim = std::min(lim, tile_room);
+    const int64_t n = consecutive(slots + i, s, lim);
+    push_run(Run{static_cast<int32_t>(s), static_cast<int32_t>(i - b_shift), static_cast<int32_t>(n)}, bs, hnd,
+             full, partial);
+    i += n;
+    chunk_room -= n;
+    if (chunk_room == 0) chunk_room = C;
+    if (hnd && (tile_room -= n) == 0) tile_room = bs;
+  }
+  return B200KV_OK;
+}
+
+// Runs of a peer pull: token i moves peer slot src[i] to local slot dst[i].  A run never crosses a
+// vLLM block on either side.  Returns B200KV_EINVAL if a source slot lies outside [0, max_src) or a
+// destination slot outside [0, max_dst); the lists then hold an unspecified prefix.
+inline int build_pull_runs(const int64_t* src, const int64_t* dst, int64_t n_tokens, int64_t max_src,
+                           int64_t max_dst, int32_t bs, bool hnd, std::vector<Run>* full,
+                           std::vector<Run>* partial) {
+  for (int64_t i = 0; i < n_tokens;) {
+    const int64_t s = src[i], d = dst[i];
+    if (out_of_range(s, max_src) || out_of_range(d, max_dst)) return B200KV_EINVAL;
+    const int64_t lim = std::min({static_cast<int64_t>(bs) - s % bs, static_cast<int64_t>(bs) - d % bs, max_src - s,
+                                  max_dst - d, n_tokens - i});
+    int64_t n = 1;
+    while (n < lim && src[i + n] == s + n && dst[i + n] == d + n) ++n;
+    push_run(Run{static_cast<int32_t>(s), static_cast<int32_t>(d), static_cast<int32_t>(n)}, bs, hnd, full, partial);
+    i += n;
+  }
+  return B200KV_OK;
+}
+
+}  // namespace b200kv

@@ -1,0 +1,281 @@
+"""Run tables (csrc/b200kv_runs.h) against the per-token rule they replace.
+
+The header is host-only: it is compiled here with g++ behind a small extern "C" wrapper and called
+through ctypes.  The reference below restates the per-token rule: token i extends the current run
+when its slot follows the run's last slot, the slot does not start a vLLM block, the op-relative
+index i - b_shift does not start a chunk and, for HND, does not start a tile; a pull run also needs
+the destination slot to follow on and not start a block.  HND runs are split into whole aligned
+tiles and the rest.  CPU only."""
+import ctypes as C
+import os
+import subprocess
+
+import numpy as np
+import pytest
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+EINVAL = -22
+
+WRAPPER = r"""
+#include "b200kv_runs.h"
+using b200kv::Run;
+
+static void out(const std::vector<Run>& v, Run* dst, int64_t* n) {
+  for (size_t i = 0; i < v.size(); ++i) dst[i] = v[i];
+  *n = static_cast<int64_t>(v.size());
+}
+
+extern "C" int op_runs(const int64_t* slots, int64_t tok_begin, int64_t tok_end, int64_t b_shift, int64_t max_slot,
+                       int32_t bs, int32_t C, int hnd, int split, Run* full, int64_t* n_full, Run* part,
+                       int64_t* n_part) {
+  std::vector<Run> f, p;
+  const int rc = b200kv::build_runs(slots, tok_begin, tok_end, b_shift, max_slot, bs, C, hnd != 0, &f,
+                                    split ? &p : nullptr);
+  out(f, full, n_full);
+  out(p, part, n_part);
+  return rc;
+}
+
+extern "C" int pull_runs(const int64_t* src, const int64_t* dst, int64_t n, int64_t max_src, int64_t max_dst,
+                         int32_t bs, int hnd, Run* full, int64_t* n_full, Run* part, int64_t* n_part) {
+  std::vector<Run> f, p;
+  const int rc = b200kv::build_pull_runs(src, dst, n, max_src, max_dst, bs, hnd != 0, &f, &p);
+  out(f, full, n_full);
+  out(p, part, n_part);
+  return rc;
+}
+"""
+
+
+@pytest.fixture(scope="module")
+def lib(tmp_path_factory):
+    d = tmp_path_factory.mktemp("runs")
+    src, so = d / "runs_wrapper.cpp", d / "librunswrapper.so"
+    src.write_text(WRAPPER)
+    subprocess.run(["g++", "-std=c++17", "-O2", "-Wall", "-Wextra", "-Werror", "-shared", "-fPIC",
+                    "-I", os.path.join(ROOT, "production-stack_b200", "csrc"), "-I", os.path.join(ROOT, "include"),
+                    str(src), "-o", str(so)], check=True)
+    return C.CDLL(str(so))
+
+
+def _p(a):
+    return a.ctypes.data_as(C.c_void_p)
+
+
+def _call(fn, args, n):
+    full, part = np.zeros((max(n, 1), 3), np.int32), np.zeros((max(n, 1), 3), np.int32)
+    nf, npart = C.c_int64(-1), C.c_int64(-1)
+    rc = fn(*args, _p(full), C.byref(nf), _p(part), C.byref(npart))
+    if rc:
+        return rc, None, None
+    return rc, [tuple(r) for r in full[:nf.value]], [tuple(r) for r in part[:npart.value]]
+
+
+def build(lib, slots, tb, te, b_shift, max_slot, bs, c, hnd, split=True):
+    slots = np.ascontiguousarray(slots, np.int64)
+    args = (_p(slots), C.c_int64(tb), C.c_int64(te), C.c_int64(b_shift), C.c_int64(max_slot), C.c_int32(bs),
+            C.c_int32(c), C.c_int(hnd), C.c_int(split))
+    return _call(lib.op_runs, args, te - tb)
+
+
+def build_pull(lib, src, dst, max_src, max_dst, bs, hnd):
+    src, dst = np.ascontiguousarray(src, np.int64), np.ascontiguousarray(dst, np.int64)
+    args = (_p(src), _p(dst), C.c_int64(len(src)), C.c_int64(max_src), C.c_int64(max_dst), C.c_int32(bs), C.c_int(hnd))
+    return _call(lib.pull_runs, args, len(src))
+
+
+def _sink(bs, hnd, split):
+    full, part = [], []
+
+    def push(r):
+        a, b, n = r
+        whole = n == bs and a % bs == 0 and b % bs == 0
+        (part if hnd and split and not whole else full).append(r)
+    return full, part, push
+
+
+def ref(slots, tb, te, b_shift, max_slot, bs, c, hnd, split=True):
+    full, part, push = _sink(bs, hnd, split)
+    cur = None
+    for i in range(tb, te):
+        s, j = int(slots[i]), i - b_shift
+        if s < 0 or s >= max_slot:
+            return EINVAL, None, None
+        if (cur and s == cur[0] + cur[2] and s % bs and j % c and not (hnd and j % bs == 0)):
+            cur[2] += 1
+        else:
+            if cur:
+                push(tuple(cur))
+            cur = [s, j, 1]
+    if cur:
+        push(tuple(cur))
+    return 0, full, part
+
+
+def ref_pull(src, dst, max_src, max_dst, bs, hnd):
+    full, part, push = _sink(bs, hnd, True)
+    cur = None
+    for s, d in zip(map(int, src), map(int, dst)):
+        if not (0 <= s < max_src and 0 <= d < max_dst):
+            return EINVAL, None, None
+        if cur and s == cur[0] + cur[2] and d == cur[1] + cur[2] and s % bs and d % bs:
+            cur[2] += 1
+        else:
+            if cur:
+                push(tuple(cur))
+            cur = [s, d, 1]
+    if cur:
+        push(tuple(cur))
+    return 0, full, part
+
+
+def block_map(blocks, n_tok, bs, start=0):
+    """vLLM slot mapping of tokens [start, start + n_tok) of a request with block table `blocks`."""
+    i = np.arange(start, start + n_tok, dtype=np.int64)
+    return np.asarray(blocks, np.int64)[i // bs] * bs + i % bs
+
+
+def random_map(rng, n_tok, nb, bs):
+    """A map made of pieces of every shape the builders meet: block tables entered mid-block, single
+    tokens, runs of consecutive slots that cross block boundaries, and repeated slots."""
+    parts, left = [], n_tok
+    while left > 0:
+        k = int(rng.integers(1, min(left, 3 * bs) + 1))
+        kind = rng.integers(0, 4)
+        if kind == 0:
+            blocks = rng.permutation(nb)[:(k + 2 * bs) // bs + 1]
+            parts.append(block_map(blocks, k, bs, start=int(rng.integers(0, bs))))
+        elif kind == 1:
+            parts.append(rng.integers(0, nb * bs, k))
+        elif kind == 2:
+            s0 = int(rng.integers(0, nb * bs - k))
+            parts.append(np.arange(s0, s0 + k))
+        else:
+            parts.append(np.full(k, rng.integers(0, nb * bs)))
+        left -= k
+    return np.concatenate(parts).astype(np.int64)
+
+
+# (bs, C): geometries make_geometry accepts, plus one whose chunk is not a whole number of blocks
+# (make_geometry refuses it today; the HND tile rule must still follow the op-relative index)
+GEOMS = [(16, 256), (16, 64), (8, 32), (16, 16), (16, 40)]
+
+
+@pytest.mark.parametrize("hnd", [False, True])
+@pytest.mark.parametrize("bs,c", GEOMS)
+def test_random_maps_match_the_per_token_rule(lib, bs, c, hnd):
+    rng = np.random.default_rng(bs * 1000 + c + hnd)
+    nb = 64
+    for _ in range(150):
+        n = int(rng.integers(1, 5 * c))
+        slots = random_map(rng, n, nb, bs)
+        tb = int(rng.integers(0, n))
+        te = int(rng.integers(tb + 1, n + 1))
+        b_shift = int(rng.integers(-c, tb + 1))          # op-relative indices stay >= 0, as in the engine
+        for split in (True, False):
+            want = ref(slots, tb, te, b_shift, nb * bs, bs, c, hnd, split)
+            assert build(lib, slots, tb, te, b_shift, nb * bs, bs, c, hnd, split) == want
+
+
+@pytest.mark.parametrize("hnd", [False, True])
+def test_batch_of_ragged_requests_matches_the_per_token_rule(lib, hnd):
+    """Store / load batches: chunk k of the op holds the k-th chunk's slots at k*C, a request's last
+    chunk is short, and chunk i of a staging batch is indexed from i*C (b_shift = k*C - i*C)."""
+    bs, c, nb = 16, 64, 256
+    rng = np.random.default_rng(7 + hnd)
+    perm = rng.permutation(nb)
+    sm, ntok, used = [], [], 0
+    for n_req in (c + 5, 2 * c, 3 * c + 1, 17, c):
+        nblk = (n_req + bs - 1) // bs
+        req = block_map(perm[used:used + nblk], n_req, bs)
+        used += nblk
+        for k in range(0, n_req, c):
+            t = req[k:k + c]
+            sm.append(np.concatenate([t, np.full(c - len(t), -1)]))
+            ntok.append(len(t))
+    sm = np.concatenate(sm)
+    for stage in (1, 3, len(ntok)):                      # staging batches of several sizes
+        for b0 in range(0, len(ntok), stage):
+            for i, k in enumerate(range(b0, min(b0 + stage, len(ntok)))):
+                tb = k * c
+                args = (sm, tb, tb + ntok[k], tb - i * c, nb * bs, bs, c, hnd)
+                got = build(lib, *args)
+                assert got[0] == 0 and got == ref(*args)
+
+
+@pytest.mark.parametrize("hnd", [False, True])
+def test_token_granular_and_shuffled_maps(lib, hnd):
+    bs, c, nb = 16, 256, 512
+    rng = np.random.default_rng(11)
+    tokens = rng.permutation(nb * bs)[:3000]                          # every token its own slot
+    shuffled = block_map(rng.permutation(nb)[:200], 3000, bs)         # whole blocks in random order
+    mid = block_map(rng.permutation(nb)[:200], 3000, bs, start=5)     # a request entered mid-block
+    for slots in (tokens, shuffled, mid):
+        for b_shift in (0, -3, 7):
+            tb = max(b_shift, 0)
+            args = (slots, tb, len(slots), b_shift, nb * bs, bs, c, hnd)
+            got = build(lib, *args)
+            assert got[0] == 0 and got == ref(*args)
+
+
+@pytest.mark.parametrize("hnd", [False, True])
+def test_pull_runs_check_both_sides(lib, hnd):
+    bs, nb_src, nb_dst = 16, 48, 64
+    rng = np.random.default_rng(3 + hnd)
+    for _ in range(200):
+        n = int(rng.integers(1, 300))
+        src = random_map(rng, n, nb_src, bs)
+        dst = random_map(rng, n, nb_dst, bs) if rng.integers(0, 2) else \
+            block_map(rng.permutation(nb_dst), n, bs, start=int(rng.integers(0, bs)))
+        got = build_pull(lib, src, dst, nb_src * bs, nb_dst * bs, bs, hnd)
+        assert got[0] == 0 and got == ref_pull(src, dst, nb_src * bs, nb_dst * bs, bs, hnd)
+    # the source side follows on but the destination does not (and the other way round)
+    src = np.arange(32, dtype=np.int64)
+    dst = np.concatenate([np.arange(100, 108), np.arange(200, 224)]).astype(np.int64)
+    for a, b in ((src, dst), (dst, src)):
+        got = build_pull(lib, a, b, 4096, 4096, bs, hnd)
+        assert got[0] == 0 and got == ref_pull(a, b, 4096, 4096, bs, hnd)
+
+
+@pytest.mark.parametrize("bad", [-1, "max"])
+@pytest.mark.parametrize("where", [0, "mid", "last"])
+def test_out_of_range_slots_are_refused(lib, bad, where):
+    bs, c, nb = 16, 64, 32
+    max_slot = nb * bs
+    slots = block_map(np.arange(nb), 200, bs)
+    pos = {0: 0, "mid": 100, "last": 199}[where]
+    slots[pos] = max_slot if bad == "max" else -1
+    for hnd in (False, True):
+        assert build(lib, slots, 0, 200, 0, max_slot, bs, c, hnd)[0] == EINVAL
+    ok = block_map(np.arange(nb), 200, bs)
+    assert build_pull(lib, slots, ok, max_slot, max_slot, bs, False)[0] == EINVAL
+    assert build_pull(lib, ok, slots, max_slot, max_slot, bs, False)[0] == EINVAL
+    # each side is checked against its own bound: slot 199 is past a bound of 199 on either side
+    assert build_pull(lib, ok, ok, 199, max_slot, bs, False)[0] == EINVAL
+    assert build_pull(lib, ok, ok, max_slot, 199, bs, False)[0] == EINVAL
+    assert build_pull(lib, ok, ok, 200, 200, bs, False)[0] == 0
+    for hnd in (False, True):       # a bound that is not a whole number of blocks
+        assert build(lib, ok, 0, 200, 0, 199, bs, c, hnd)[0] == EINVAL
+        assert build(lib, ok, 0, 199, 0, 199, bs, c, hnd) == ref(ok, 0, 199, 0, 199, bs, c, hnd)
+    # slots that keep counting up past the bound: the first one past it starts a run of its own
+    up = np.arange(max_slot - 20, max_slot + 5, dtype=np.int64)
+    for hnd in (False, True):
+        assert build(lib, up, 0, len(up), 0, max_slot, bs, c, hnd)[0] == EINVAL
+        assert build(lib, up, 0, 20, 0, max_slot, bs, c, hnd) == ref(up, 0, 20, 0, max_slot, bs, c, hnd)
+    assert build_pull(lib, up, up - 100, max_slot, max_slot, bs, False)[0] == EINVAL
+    assert build_pull(lib, up - 100, up, max_slot, max_slot, bs, False)[0] == EINVAL
+    # tokens outside [tok_begin, tok_end) are not read
+    if where == "last":
+        assert build(lib, slots, 0, 199, 0, max_slot, bs, c, False)[0] == 0
+
+
+def test_bench_shape_gives_one_run_per_block(lib):
+    """The device-resident step of bench.py: 16 sessions x 2048 tokens over shuffled 16-token blocks."""
+    bs, c, nb, n = 16, 256, 8192, 16 * 2048
+    perm = np.random.default_rng(1234).permutation(nb)
+    slots = np.concatenate([block_map(perm[s * 128:(s + 1) * 128], 2048, bs) for s in range(16)])
+    rc, full, part = build(lib, slots, 0, n, 0, nb * bs, bs, c, False)
+    assert rc == 0 and part == [] and len(full) == 2048
+    assert all(r[2] == 16 for r in full)
+    assert [r[1] for r in full] == list(range(0, n, 16))
+    assert [r[0] for r in full] == [int(slots[i]) for i in range(0, n, 16)]
