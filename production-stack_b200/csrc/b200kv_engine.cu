@@ -56,9 +56,11 @@ void set_err(const char* what, cudaError_t e, int line) {
   } while (0)
 
 constexpr int kTableSlots = 16;
-constexpr size_t kTableBytes = 1u << 20;
 constexpr int kMaxPeers = 64;
 constexpr uint32_t kStageMax = 32u << 10;
+
+// kernel-time slots of b200kv_last_kernel_ms: stores and gathers, loads and scatters, peer pulls
+enum TimingSlot { kTimeGather = 0, kTimeScatter = 1, kTimePull = 2, kTimingSlots = 3 };
 
 struct StageSlot {
   cudaEvent_t free_ev = nullptr;  // recorded when the last consumer of this slot is done
@@ -101,11 +103,11 @@ void CUDART_CB op_host_cb(void* p) {
   op->host_done.store(1, std::memory_order_release);
 }
 
-// Undoes what a store / load had taken when it leaves early (argument the table cannot hold, a failed
-// CUDA call): reserved-but-uncommitted pool slots are aborted (otherwise later stores of those keys see
-// -EEXIST until the stale-writer reclaim), pinned chunks are released (otherwise they can never be
+// Undoes what a store / load / pull had taken when it leaves early (argument the table cannot hold, a
+// failed CUDA call): reserved-but-uncommitted pool slots are aborted (otherwise later stores of those keys
+// see -EEXIST until the stale-writer reclaim), pinned chunks are released (otherwise they can never be
 // evicted), and the op's events are destroyed.  The engine's streams are drained first, so no copy into
-// or out of those slots is still in flight.
+// or out of those slots is still in flight and no host callback enqueued for the op can still run.
 struct OpGuard {
   b200kv_ctx* ctx;
   cudaStream_t s[4];
@@ -207,6 +209,7 @@ struct b200kv_ctx {
   std::mutex mu;
 
   cudaStream_t s_gather = nullptr, s_d2h = nullptr, s_h2d = nullptr, s_scatter = nullptr;
+  cudaEvent_t fence = nullptr;          // stream_wait's event
   uint64_t* d_bases = nullptr;
   bool kv_registered = false;
   std::vector<const void*> h_k, h_v;
@@ -229,14 +232,13 @@ struct b200kv_ctx {
   struct Timing {
     std::vector<std::pair<cudaEvent_t, cudaEvent_t>> ev;
     size_t used = 0;
-  } timing[3];
+  } timing[kTimingSlots];
 
   b200kv_engine_stats stats{};
 
   // bulk-kernel launch shape
   int S = 2, LAG = 1, ctas_per_sm = 1;  // B200KV_STAGES / B200KV_LAG / B200KV_CTAS_PER_SM (tools/sweep.py)
   int fp8_threads = 256;                // B200KV_FP8_THREADS: CTA width of the FP8 store kernel
-  bool fp8_two_pass = false;            // B200KV_FP8_2PASS=1: smem-free two-pass store kernel (experimental, slower)
   int fp8_store_ver = 3;                // B200KV_FP8_STORE: 3 = persistent warp-specialised kernel (default), 1 = cluster kernel
   void* d_tmaps = nullptr;              // one CUtensorMap per plane (NHD pages: strided [bs][D] boxes for the FP8 store)
   std::string tmap_status = "not built";
@@ -267,45 +269,67 @@ int env_int(const char* name, int dflt) {
   return (v && *v) ? std::atoi(v) : dflt;
 }
 
-// ---- run construction (host): b200kv_runs.h --------------------------------------------------
-int op_runs(const b200kv_ctx* ctx, const int64_t* slots, int64_t tok_begin, int64_t tok_end, int64_t b_shift,
-            std::vector<Run>* full, std::vector<Run>* partial) {
+// ---- run tables: built by b200kv_runs.h, staged through the table ring --------------------------
+int op_table(const b200kv_ctx* ctx, const int64_t* slots, const std::vector<Span>& spans, OpTable* t) {
   const Geometry& g = ctx->g;
-  return build_runs(slots, tok_begin, tok_end, b_shift, static_cast<int64_t>(ctx->cfg.n_blocks) * g.bs,
-                    static_cast<int32_t>(g.bs), static_cast<int32_t>(g.C), g.hnd, full, partial);
+  return build_op_table(slots, spans.data(), spans.size(), static_cast<int64_t>(ctx->cfg.n_blocks) * g.bs,
+                        static_cast<int32_t>(g.bs), static_cast<int32_t>(g.C), ctx->cfg.format == B200KV_FMT_RAW,
+                        g.hnd, t);
 }
 
-// ---- table ring ------------------------------------------------------------------------------
+// a staged table: its ring slot and its arrays in device memory
 struct TableView {
   TableSlot* slot;
-  size_t runs_off, addrs_off, offs_off, bytes;
+  const Run* runs;
+  const uint64_t* chunk_addrs;
+  const uint32_t* full_off;
 };
 
-int table_acquire(b200kv_ctx* ctx, size_t n_runs, size_t n_chunks, TableView* tv) {
-  const size_t runs_bytes = (n_runs * sizeof(Run) + 15) / 16 * 16;
-  const size_t addrs_bytes = (n_chunks * 8 + 15) / 16 * 16;
-  const size_t offs_bytes = ((n_chunks + 1) * 4 + 15) / 16 * 16;
-  const size_t total = runs_bytes + addrs_bytes + offs_bytes;
-  if (total > kTableBytes) return B200KV_EINVAL;  // op too large: caller must split
-  TableSlot& t = ctx->tables[ctx->table_next];
+// Takes the next slot of the table ring, fills it with `t` and chunk_addrs[0, t.n_chunks()) and uploads it
+// on `s`.  A table over kTableBytes is refused before anything is enqueued.
+int stage_table(b200kv_ctx* ctx, const OpTable& t, const uint64_t* chunk_addrs, cudaStream_t s, TableView* tv) {
+  const uint32_t n_chunks = t.n_chunks();
+  TableLayout l;
+  if (table_layout(t.runs.size(), n_chunks, &l)) return B200KV_EINVAL;  // op too large: caller must split
+  TableSlot& ts = ctx->tables[ctx->table_next];
   ctx->table_next = (ctx->table_next + 1) % kTableSlots;
-  if (t.used) {  // host must not overwrite a table whose upload / readers are still in flight
-    CU_TRY(cudaEventSynchronize(t.ev));
-    CU_TRY(cudaEventSynchronize(t.done_ev));
+  if (ts.used) {  // host must not overwrite a table whose upload / readers are still in flight
+    CU_TRY(cudaEventSynchronize(ts.ev));
+    CU_TRY(cudaEventSynchronize(ts.done_ev));
   }
-  tv->slot = &t;
-  tv->runs_off = 0;
-  tv->addrs_off = runs_bytes;
-  tv->offs_off = runs_bytes + addrs_bytes;
-  tv->bytes = total;
+  std::memcpy(ts.host + l.runs_off, t.runs.data(), t.runs.size() * sizeof(Run));
+  std::memcpy(ts.host + l.addrs_off, chunk_addrs, n_chunks * sizeof(uint64_t));
+  std::memcpy(ts.host + l.offs_off, t.full_off.data(), (n_chunks + 1) * sizeof(uint32_t));
+  CU_TRY(cudaMemcpyAsync(ts.dev, ts.host, l.bytes, cudaMemcpyHostToDevice, s));
+  CU_TRY(cudaEventRecord(ts.ev, s));
+  ts.used = true;
+  ctx->stats.h2d_bytes += l.bytes;
+  tv->slot = &ts;
+  tv->runs = reinterpret_cast<const Run*>(ts.dev + l.runs_off);
+  tv->chunk_addrs = reinterpret_cast<const uint64_t*>(ts.dev + l.addrs_off);
+  tv->full_off = reinterpret_cast<const uint32_t*>(ts.dev + l.offs_off);
   return B200KV_OK;
 }
 
-int table_upload(b200kv_ctx* ctx, const TableView& tv, cudaStream_t s) {
-  CU_TRY(cudaMemcpyAsync(tv.slot->dev, tv.slot->host, tv.bytes, cudaMemcpyHostToDevice, s));
-  CU_TRY(cudaEventRecord(tv.slot->ev, s));
-  tv.slot->used = true;
-  ctx->stats.h2d_bytes += tv.bytes;
+// Makes `waiter` wait for the work enqueued on `signaller` so far.  cudaStreamWaitEvent takes the event's
+// current record, so one event serves every wait made under ctx->mu.
+int stream_wait(b200kv_ctx* ctx, cudaStream_t waiter, cudaStream_t signaller) {
+  CU_TRY(cudaEventRecord(ctx->fence, signaller));
+  CU_TRY(cudaStreamWaitEvent(waiter, ctx->fence, 0));
+  return B200KV_OK;
+}
+
+// Every chunk holds 1..C tokens and every slot of chunk c, slot_mapping[c*C, c*C + chunk_tokens[c]), lies in
+// [0, n_blocks*bs).  Ops check this before they reserve or pin anything, so a malformed mapping takes nothing.
+int check_chunk_slots(const b200kv_ctx* ctx, const int64_t* slot_mapping, const int32_t* chunk_tokens,
+                      int32_t n_chunks) {
+  const int64_t max_slot = static_cast<int64_t>(ctx->cfg.n_blocks) * ctx->g.bs;
+  for (int32_t c = 0; c < n_chunks; ++c) {
+    if (chunk_tokens[c] <= 0 || chunk_tokens[c] > static_cast<int32_t>(ctx->g.C)) return B200KV_EINVAL;
+    const int64_t* sm = slot_mapping + static_cast<int64_t>(c) * ctx->g.C;
+    for (int32_t i = 0; i < chunk_tokens[c]; ++i)
+      if (out_of_range(sm[i], max_slot)) return B200KV_EINVAL;
+  }
   return B200KV_OK;
 }
 
@@ -331,37 +355,28 @@ int timing_end(b200kv_ctx* ctx, int which, cudaStream_t s) {
 }
 
 // ---- kernel launches ---------------------------------------------------------------------------
-template <int MODE, int S, int LAG>
-int launch_bulk_t(b200kv_ctx* ctx, const CopyParams& p, cudaStream_t s) {
-  const size_t smem = 256 + static_cast<size_t>(S) * ctx->stage_bytes;
-  static bool attr_set[8] = {false};  // per device ordinal (<=8 GPUs per box)
-  const int dev = ctx->cfg.device & 7;
-  if (!attr_set[dev]) {
-    CU_TRY(cudaFuncSetAttribute(kv_bulk_copy_kernel<MODE, S, LAG>,
-                                cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set[dev] = true;
-  }
-  uint32_t grid = static_cast<uint32_t>(ctx->sm_count * ctx->ctas_per_sm);
-  grid = std::min(grid, p.total_units);
-  if (grid == 0) return B200KV_OK;
-  kv_bulk_copy_kernel<MODE, S, LAG><<<grid, 32, smem, s>>>(p, ctx->stage_bytes);
+// the end of every launch: a launch error fails the op, and stats count the launches
+int launched(b200kv_ctx* ctx) {
   CU_TRY(cudaGetLastError());
   ++ctx->stats.n_kernel_launches;
   return B200KV_OK;
 }
 
+typedef void (*BulkKernel)(CopyParams, uint32_t);
+
+// the bulk kernel built for a B200KV_STAGES / B200KV_LAG pair; null for a pair that is not built
 template <int MODE>
-int launch_bulk(b200kv_ctx* ctx, const CopyParams& p, cudaStream_t s) {
-  switch (ctx->S * 10 + ctx->LAG) {
-    case 21: return launch_bulk_t<MODE, 2, 1>(ctx, p, s);
-    case 31: return launch_bulk_t<MODE, 3, 1>(ctx, p, s);
-    case 32: return launch_bulk_t<MODE, 3, 2>(ctx, p, s);
-    case 41: return launch_bulk_t<MODE, 4, 1>(ctx, p, s);
-    case 42: return launch_bulk_t<MODE, 4, 2>(ctx, p, s);
-    case 43: return launch_bulk_t<MODE, 4, 3>(ctx, p, s);
-    case 63: return launch_bulk_t<MODE, 6, 3>(ctx, p, s);
-    case 64: return launch_bulk_t<MODE, 6, 4>(ctx, p, s);
-    default: return B200KV_EINVAL;
+BulkKernel bulk_kernel(int S, int LAG) {
+  switch (S * 10 + LAG) {
+    case 21: return kv_bulk_copy_kernel<MODE, 2, 1>;
+    case 31: return kv_bulk_copy_kernel<MODE, 3, 1>;
+    case 32: return kv_bulk_copy_kernel<MODE, 3, 2>;
+    case 41: return kv_bulk_copy_kernel<MODE, 4, 1>;
+    case 42: return kv_bulk_copy_kernel<MODE, 4, 2>;
+    case 43: return kv_bulk_copy_kernel<MODE, 4, 3>;
+    case 63: return kv_bulk_copy_kernel<MODE, 6, 3>;
+    case 64: return kv_bulk_copy_kernel<MODE, 6, 4>;
+    default: return nullptr;
   }
 }
 
@@ -372,11 +387,16 @@ int launch_copy(b200kv_ctx* ctx, const CopyParams& p, cudaStream_t s) {
     grid = std::min(grid, p.total_units);
     if (grid == 0) return B200KV_OK;
     kv_ldg_copy_kernel<MODE><<<grid, 256, 0, s>>>(p);
-    CU_TRY(cudaGetLastError());
-    ++ctx->stats.n_kernel_launches;
-    return B200KV_OK;
+    return launched(ctx);
   }
-  return launch_bulk<MODE>(ctx, p, s);
+  const BulkKernel kernel = bulk_kernel<MODE>(ctx->S, ctx->LAG);
+  if (!kernel) return B200KV_EINVAL;
+  const size_t smem = 256 + static_cast<size_t>(ctx->S) * ctx->stage_bytes;
+  uint32_t grid = static_cast<uint32_t>(ctx->sm_count * ctx->ctas_per_sm);
+  grid = std::min(grid, p.total_units);
+  if (grid == 0) return B200KV_OK;
+  kernel<<<grid, 32, smem, s>>>(p, ctx->stage_bytes);
+  return launched(ctx);
 }
 
 // format tag recorded with a chunk: a pool shared by engines of different tile order or codec
@@ -394,68 +414,55 @@ PagedSide local_side(const b200kv_ctx* ctx) {
   return s;
 }
 
-CopyParams make_copy_params(const b200kv_ctx* ctx, const uint8_t* dev_table, const TableView& tv,
-                            size_t run_begin, size_t n_runs, uint32_t plane_begin = 0, uint32_t n_planes = 0) {
+// Full runs [f0, f0 + nf) of the table go to the bulk (or LDG) kernel, HND partial-tile runs [p0, p0 + np)
+// to kv_hnd_partial_kernel.  `peer` non-null selects the pull source.
+template <int MODE>
+int launch_copy_runs(b200kv_ctx* ctx, const TableView& tv, size_t f0, size_t nf, size_t p0, size_t np,
+                     cudaStream_t s, const Peer* peer, uint32_t plane_begin, uint32_t n_planes) {
   CopyParams p{};
   p.paged = local_side(ctx);
   p.peer = p.paged;
-  p.chunk.chunk_addrs = reinterpret_cast<const uint64_t*>(dev_table + tv.addrs_off);
+  if (peer) {
+    p.peer.bases = peer->d_bases;
+    p.peer.block_stride = peer->block_stride;
+  }
+  p.chunk.chunk_addrs = tv.chunk_addrs;
   p.chunk.slab_bytes = ctx->g.slab_bytes;
   p.chunk.chunk_tokens = ctx->g.C;
   p.chunk.token_bytes = ctx->g.fmt_token_bytes;
-  p.runs = reinterpret_cast<const Run*>(dev_table + tv.runs_off) + run_begin;
-  p.n_runs = static_cast<uint32_t>(n_runs);
+  p.runs = tv.runs + f0;
+  p.n_runs = static_cast<uint32_t>(nf);
   p.n_planes = n_planes ? n_planes : ctx->g.planes;
   p.plane_begin = plane_begin;
   p.pieces = ctx->pieces;
   p.piece_tokens = ctx->piece_tokens;
   p.total_units = p.n_runs * p.n_planes * p.pieces;
-  return p;
-}
-
-template <int MODE>
-int launch_hnd_partial(b200kv_ctx* ctx, const CopyParams& cp, const Run* runs, uint32_t n_runs, cudaStream_t s) {
-  if (n_runs == 0) return B200KV_OK;
-  HndParams p{};
-  p.paged = cp.paged;
-  p.peer = cp.peer;
-  p.chunk = cp.chunk;
-  p.runs = runs;
-  p.n_runs = n_runs;
-  p.n_planes = cp.n_planes;
-  p.plane_begin = cp.plane_begin;
-  p.n_heads = ctx->g.H;
-  p.row_bytes = ctx->g.row_bytes;
-  p.total_units = n_runs * p.n_planes * p.n_heads;
-  const uint32_t grid = std::min<uint32_t>(p.total_units, static_cast<uint32_t>(ctx->sm_count) * 16u);
-  kv_hnd_partial_kernel<MODE><<<grid, 128, 0, s>>>(p);
-  CU_TRY(cudaGetLastError());
-  ++ctx->stats.n_kernel_launches;
-  return B200KV_OK;
-}
-
-// runs [run_begin, +n_full) are whole tiles (or anything, for NHD); the next n_partial are HND
-// partial-tile runs.  `peer` non-null selects the pull source.
-template <int MODE>
-int launch_copy_runs(b200kv_ctx* ctx, const uint8_t* dev_table, const TableView& tv, size_t run_begin,
-                     size_t n_full, size_t n_partial, cudaStream_t s, const Peer* peer = nullptr,
-                     uint32_t plane_begin = 0, uint32_t n_planes = 0) {
-  CopyParams p = make_copy_params(ctx, dev_table, tv, run_begin, n_full, plane_begin, n_planes);
-  if (peer) {
-    p.peer.bases = peer->d_bases;
-    p.peer.block_stride = peer->block_stride;
+  if (nf) {
+    const int rc = launch_copy<MODE>(ctx, p, s);
+    if (rc) return rc;
   }
-  int rc = B200KV_OK;
-  if (n_full) rc = launch_copy<MODE>(ctx, p, s);
-  if (rc) return rc;
-  return launch_hnd_partial<MODE>(ctx, p, p.runs + n_full, static_cast<uint32_t>(n_partial), s);
+  if (np == 0) return B200KV_OK;
+  HndParams h{};
+  h.paged = p.paged;
+  h.peer = p.peer;
+  h.chunk = p.chunk;
+  h.runs = tv.runs + p0;
+  h.n_runs = static_cast<uint32_t>(np);
+  h.n_planes = p.n_planes;
+  h.plane_begin = p.plane_begin;
+  h.n_heads = ctx->g.H;
+  h.row_bytes = ctx->g.row_bytes;
+  h.total_units = h.n_runs * h.n_planes * h.n_heads;
+  const uint32_t grid = std::min<uint32_t>(h.total_units, static_cast<uint32_t>(ctx->sm_count) * 16u);
+  kv_hnd_partial_kernel<MODE><<<grid, 128, 0, s>>>(h);
+  return launched(ctx);
 }
 
 // Persistent FP8 store (kv_fp8_store3_kernel) when every chunk of the batch is a sequence of whole, block-aligned
 // runs (the last possibly short).  Returns 1 if it launched, 0 if the batch is not eligible, < 0 on error.
-static int try_launch_fp8_store3(b200kv_ctx* ctx, const uint8_t* dev_table, const TableView& tv, uint32_t n_chunks,
-                                 const uint32_t* chunk_ntok, cudaStream_t s) {
+int try_launch_fp8_store3(b200kv_ctx* ctx, const OpTable& t, const TableView& tv, cudaStream_t s) {
   const Geometry& g = ctx->g;
+  const uint32_t n_chunks = t.n_chunks();
   const uint32_t head_bytes = g.D * 2, rv = head_bytes >> 4;
   const uint64_t unit_bytes = static_cast<uint64_t>(g.C) * head_bytes;
   if (ctx->fp8_store_ver != 3 || g.elem != 2 || unit_bytes > kS3MaxUnitBytes || (head_bytes & 15) || rv == 0 ||
@@ -464,11 +471,12 @@ static int try_launch_fp8_store3(b200kv_ctx* ctx, const uint8_t* dev_table, cons
     return 0;
   const bool use_tmap = !g.hnd || env_int("B200KV_FP8_TMAP_HND", 0);
   if (use_tmap && (!ctx->d_tmaps || ctx->tmap_status != "ok")) return 0;
-  const Run* runs = reinterpret_cast<const Run*>(tv.slot->host + tv.runs_off);
-  const uint32_t* offs = reinterpret_cast<const uint32_t*>(tv.slot->host + tv.offs_off);
+  const Run* runs = t.runs.data();
+  const uint32_t* offs = t.full_off.data();
   for (uint32_t c = 0; c < n_chunks; ++c) {
     const uint32_t base = c * g.C;
-    const uint32_t n_valid = chunk_ntok[c];
+    uint32_t n_valid = 0;   // the chunk's tokens: its runs cover them
+    for (uint32_t r = offs[c]; r < offs[c + 1]; ++r) n_valid += static_cast<uint32_t>(runs[r].n);
     if (n_valid == 0 || n_valid > g.C) return 0;
     const uint32_t nb = (n_valid + g.bs - 1) / g.bs;
     if (offs[c + 1] - offs[c] != nb) return 0;
@@ -481,9 +489,9 @@ static int try_launch_fp8_store3(b200kv_ctx* ctx, const uint8_t* dev_table, cons
   }
   Fp8Store3Params p{};
   p.paged = local_side(ctx);
-  p.runs = reinterpret_cast<const Run*>(dev_table + tv.runs_off);
-  p.chunk_run_off = reinterpret_cast<const uint32_t*>(dev_table + tv.offs_off);
-  p.chunk_addrs = reinterpret_cast<const uint64_t*>(dev_table + tv.addrs_off);
+  p.runs = tv.runs;
+  p.chunk_run_off = tv.full_off;
+  p.chunk_addrs = tv.chunk_addrs;
   p.tmaps = use_tmap ? ctx->d_tmaps : nullptr;
   p.n_chunks = n_chunks;
   p.n_planes = g.planes;
@@ -496,37 +504,28 @@ static int try_launch_fp8_store3(b200kv_ctx* ctx, const uint8_t* dev_table, cons
   p.hnd = g.hnd ? 1u : 0u;
   p.total_units = n_chunks * g.planes * g.H;
   const size_t smem = static_cast<size_t>(kS3Stages) * unit_bytes;
-  static bool attr_set[8] = {false};
-  const int dev = ctx->cfg.device & 7;
-  if (!attr_set[dev]) {
-    CU_TRY(cudaFuncSetAttribute(kv_fp8_store3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kS3Stages * kS3MaxUnitBytes));
-    attr_set[dev] = true;
-  }
   const uint32_t grid = std::min<uint32_t>(p.total_units, static_cast<uint32_t>(ctx->sm_count));
   if (grid == 0) return 1;
   kv_fp8_store3_kernel<<<grid, kS3Threads, smem, s>>>(p);
-  CU_TRY(cudaGetLastError());
-  ++ctx->stats.n_kernel_launches;
-  return 1;
+  const int rc = launched(ctx);
+  return rc ? rc : 1;
 }
 
-// chunk_ntok[c] = tokens of chunk c of this launch (chunks of several requests may be partial anywhere)
-int launch_fp8_store(b200kv_ctx* ctx, const uint8_t* dev_table, const TableView& tv,
-                     uint32_t n_chunks, const uint32_t* chunk_ntok, cudaStream_t s) {
+// Every chunk of the table; chunks of several requests may be partial anywhere.
+int launch_fp8_store(b200kv_ctx* ctx, const OpTable& t, const TableView& tv, cudaStream_t s) {
   {
-    const int rc3 = try_launch_fp8_store3(ctx, dev_table, tv, n_chunks, chunk_ntok, s);
+    const int rc3 = try_launch_fp8_store3(ctx, t, tv, s);
     if (rc3 != 0) return rc3 < 0 ? rc3 : B200KV_OK;
   }
-  const uint32_t n_tokens = 0;  // unused by the kernels (see above)
-  Fp8StoreParams p{};
+  const uint32_t n_chunks = t.n_chunks();
+  Fp8StoreParams p{};   // n_tokens stays 0: unused (see above)
   p.paged = local_side(ctx);
-  p.runs = reinterpret_cast<const Run*>(dev_table + tv.runs_off);
-  p.chunk_run_off = reinterpret_cast<const uint32_t*>(dev_table + tv.offs_off);
-  p.chunk_addrs = reinterpret_cast<const uint64_t*>(dev_table + tv.addrs_off);
+  p.runs = tv.runs;
+  p.chunk_run_off = tv.full_off;
+  p.chunk_addrs = tv.chunk_addrs;
   p.n_chunks = n_chunks;
   p.n_planes = ctx->g.planes;
   p.chunk_tokens = ctx->g.C;
-  p.n_tokens = n_tokens;
   p.n_heads = ctx->g.H;
   p.head_bytes = ctx->g.D * 2;
   p.slab_q_bytes = ctx->g.slab_bytes;
@@ -536,28 +535,17 @@ int launch_fp8_store(b200kv_ctx* ctx, const uint8_t* dev_table, const TableView&
   if (smem > 200 * 1024) return B200KV_ENOTSUP;
   const uint32_t grid = kCluster * n_chunks * ctx->g.planes;
   if (grid == 0) return B200KV_OK;
-  static bool attr_set[8] = {false};
-  const int dev = ctx->cfg.device & 7;
-  if (!attr_set[dev]) {
-    CU_TRY(cudaFuncSetAttribute(kv_fp8_store_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    CU_TRY(cudaFuncSetAttribute(kv_fp8_store_kernel<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    attr_set[dev] = true;
-  }
-  if (ctx->fp8_two_pass && ctx->g.C / kCluster <= static_cast<uint32_t>(kMaxWindow)) kv_fp8_store2_kernel<<<grid, 256, 0, s>>>(p);
-  else if (ctx->fp8_threads == 512) kv_fp8_store_kernel<512><<<grid, 512, smem, s>>>(p);
+  if (ctx->fp8_threads == 512) kv_fp8_store_kernel<512><<<grid, 512, smem, s>>>(p);
   else kv_fp8_store_kernel<256><<<grid, 256, smem, s>>>(p);
-  CU_TRY(cudaGetLastError());
-  ++ctx->stats.n_kernel_launches;
-  return B200KV_OK;
+  return launched(ctx);
 }
 
-int launch_fp8_load(b200kv_ctx* ctx, const uint8_t* dev_table, const TableView& tv,
-                    size_t run_begin, size_t n_runs, cudaStream_t s, uint32_t plane_begin = 0,
-                    uint32_t n_planes = 0) {
+int launch_fp8_load(b200kv_ctx* ctx, const TableView& tv, size_t run_begin, size_t n_runs, cudaStream_t s,
+                    uint32_t plane_begin, uint32_t n_planes) {
   Fp8LoadParams p{};
   p.paged = local_side(ctx);
-  p.runs = reinterpret_cast<const Run*>(dev_table + tv.runs_off) + run_begin;
-  p.chunk_addrs = reinterpret_cast<const uint64_t*>(dev_table + tv.addrs_off);
+  p.runs = tv.runs + run_begin;
+  p.chunk_addrs = tv.chunk_addrs;
   p.n_runs = static_cast<uint32_t>(n_runs);
   p.n_planes = n_planes ? n_planes : ctx->g.planes;
   p.plane_begin = plane_begin;
@@ -573,18 +561,15 @@ int launch_fp8_load(b200kv_ctx* ctx, const uint8_t* dev_table, const TableView& 
   uint32_t grid = std::min<uint32_t>(p.total_units, static_cast<uint32_t>(ctx->sm_count) * 8u);
   if (grid == 0) return B200KV_OK;
   kv_fp8_load_kernel<<<grid, kFp8Threads, smem, s>>>(p);
-  CU_TRY(cudaGetLastError());
-  ++ctx->stats.n_kernel_launches;
-  return B200KV_OK;
+  return launched(ctx);
 }
 
-// chunk-side copy between staging and the pinned pool; partial chunks move only their tokens.
-int launch_q4(b200kv_ctx* ctx, bool store, const uint8_t* dev_table, const TableView& tv, size_t run_begin,
-              size_t n_runs, cudaStream_t s, uint32_t plane_begin = 0, uint32_t n_planes = 0) {
+int launch_q4(b200kv_ctx* ctx, bool store, const TableView& tv, size_t run_begin, size_t n_runs, cudaStream_t s,
+              uint32_t plane_begin, uint32_t n_planes) {
   Q4Params p{};
   p.paged = local_side(ctx);
-  p.runs = reinterpret_cast<const Run*>(dev_table + tv.runs_off) + run_begin;
-  p.chunk_addrs = reinterpret_cast<const uint64_t*>(dev_table + tv.addrs_off);
+  p.runs = tv.runs + run_begin;
+  p.chunk_addrs = tv.chunk_addrs;
   p.n_runs = static_cast<uint32_t>(n_runs);
   p.n_planes = n_planes ? n_planes : ctx->g.planes;
   p.plane_begin = plane_begin;
@@ -599,54 +584,49 @@ int launch_q4(b200kv_ctx* ctx, bool store, const uint8_t* dev_table, const Table
   if (grid == 0) return B200KV_OK;
   if (store) kv_q4_store_kernel<<<grid, 256, 0, s>>>(p);
   else kv_q4_load_kernel<<<grid, 256, 0, s>>>(p);
-  CU_TRY(cudaGetLastError());
-  ++ctx->stats.n_kernel_launches;
-  return B200KV_OK;
+  return launched(ctx);
 }
 
-int copy_chunk(b200kv_ctx* ctx, void* dst, const void* src, uint32_t n_tok, cudaMemcpyKind kind,
-               cudaStream_t s) {
-  const Geometry& g = ctx->g;
-  uint64_t moved;
-  if (n_tok == g.C) {
-    CU_TRY(cudaMemcpyAsync(dst, src, g.chunk_bytes, kind, s));
-    moved = g.chunk_bytes;
-  } else {
-    // HND keeps whole tiles: a ragged tail still occupies its last tile across all heads
-    const uint32_t tok_span = (g.hnd && ctx->cfg.format != B200KV_FMT_Q4) ? (n_tok + g.bs - 1) / g.bs * g.bs : n_tok;
-    const size_t width = static_cast<size_t>(tok_span) * g.fmt_token_bytes;
-    CU_TRY(cudaMemcpy2DAsync(dst, g.slab_bytes, src, g.slab_bytes, width, g.planes, kind, s));
-    moved = width * g.planes;
-    if (ctx->cfg.format == B200KV_FMT_FP8) {
-      const size_t sb = static_cast<size_t>(g.planes) * g.H * sizeof(float);
-      CU_TRY(cudaMemcpyAsync(static_cast<uint8_t*>(dst) + g.scales_off,
-                             static_cast<const uint8_t*>(src) + g.scales_off, sb, kind, s));
-      moved += sb;
-    }
+// Launches the kernels that move chunks [c0, c1) of table t, planes [pb, pb + np) (np == 0: every plane), in
+// direction `mode`.  A pull copies pages to pages whatever the chunk format.  The FP8 store always takes the
+// whole table.
+int launch_op(b200kv_ctx* ctx, CopyMode mode, const OpTable& t, const TableView& tv, uint32_t c0, uint32_t c1,
+              cudaStream_t s, uint32_t pb = 0, uint32_t np = 0, const Peer* peer = nullptr) {
+  const size_t f0 = t.full_off[c0], nf = t.full_off[c1] - f0;
+  const int fmt = mode == kPull ? B200KV_FMT_RAW : ctx->cfg.format;
+  if (fmt == B200KV_FMT_FP8)
+    return mode == kStore ? launch_fp8_store(ctx, t, tv, s) : launch_fp8_load(ctx, tv, f0, nf, s, pb, np);
+  if (fmt == B200KV_FMT_Q4) return launch_q4(ctx, mode == kStore, tv, f0, nf, s, pb, np);
+  const size_t p0 = t.n_full() + t.part_off[c0], n_part = t.part_off[c1] - t.part_off[c0];
+  switch (mode) {
+    case kStore: return launch_copy_runs<kStore>(ctx, tv, f0, nf, p0, n_part, s, peer, pb, np);
+    case kLoad: return launch_copy_runs<kLoad>(ctx, tv, f0, nf, p0, n_part, s, peer, pb, np);
+    default: return launch_copy_runs<kPull>(ctx, tv, f0, nf, p0, n_part, s, peer, pb, np);
   }
-  if (kind == cudaMemcpyDeviceToHost) ctx->stats.d2h_bytes += moved;
-  else ctx->stats.h2d_bytes += moved;
-  return B200KV_OK;
 }
 
-// planes [pb, pb+np) of one chunk between the pinned pool and staging (layer-wise loads); the
-// FP8 scales travel once, with the first group.
-int copy_chunk_planes(b200kv_ctx* ctx, void* dst, const void* src, uint32_t n_tok, uint32_t pb, uint32_t np,
-                      bool with_scales, cudaMemcpyKind kind, cudaStream_t s) {
+// Planes [pb, pb + np) of one chunk between the pinned pool and staging; np == 0 moves the whole chunk, as
+// one copy of chunk_bytes when the chunk is full.  Partial chunks move only their tokens.  The FP8 scales
+// travel with a whole chunk, and with a plane range when `with_scales` (the first group of a layer-wise load).
+int copy_chunk_planes(b200kv_ctx* ctx, void* dst, const void* src, uint32_t n_tok, cudaMemcpyKind kind,
+                      cudaStream_t s, uint32_t pb = 0, uint32_t np = 0, bool with_scales = true) {
   const Geometry& g = ctx->g;
+  const bool whole = np == 0 && n_tok == g.C;
+  if (np == 0) np = g.planes;
   uint8_t* d = static_cast<uint8_t*>(dst) + static_cast<uint64_t>(pb) * g.slab_bytes;
   const uint8_t* sp = static_cast<const uint8_t*>(src) + static_cast<uint64_t>(pb) * g.slab_bytes;
   uint64_t moved;
   if (n_tok == g.C) {
-    moved = static_cast<uint64_t>(np) * g.slab_bytes;
+    moved = whole ? g.chunk_bytes : static_cast<uint64_t>(np) * g.slab_bytes;
     CU_TRY(cudaMemcpyAsync(d, sp, moved, kind, s));
   } else {
+    // HND keeps whole tiles: a ragged tail still occupies its last tile across all heads
     const uint32_t tok_span = (g.hnd && ctx->cfg.format != B200KV_FMT_Q4) ? (n_tok + g.bs - 1) / g.bs * g.bs : n_tok;
     const size_t width = static_cast<size_t>(tok_span) * g.fmt_token_bytes;
     CU_TRY(cudaMemcpy2DAsync(d, g.slab_bytes, sp, g.slab_bytes, width, np, kind, s));
     moved = width * np;
   }
-  if (with_scales && ctx->cfg.format == B200KV_FMT_FP8) {
+  if (with_scales && !whole && ctx->cfg.format == B200KV_FMT_FP8) {
     const size_t sb = static_cast<size_t>(g.planes) * g.H * sizeof(float);
     CU_TRY(cudaMemcpyAsync(static_cast<uint8_t*>(dst) + g.scales_off, static_cast<const uint8_t*>(src) + g.scales_off,
                            sb, kind, s));
@@ -862,7 +842,6 @@ static int engine_create_impl(const b200kv_engine_config* cfg, b200kv_pool* pool
   ctx->LAG = env_int("B200KV_LAG", ctx->S / 2);
   ctx->ctas_per_sm = cfg->ctas_per_sm > 0 ? cfg->ctas_per_sm : env_int("B200KV_CTAS_PER_SM", 1);
   ctx->fp8_threads = env_int("B200KV_FP8_THREADS", 256) == 512 ? 512 : 256;
-  ctx->fp8_two_pass = env_int("B200KV_FP8_2PASS", 0) != 0;
   ctx->fp8_store_ver = env_int("B200KV_FP8_STORE", 3);
   const uint32_t stage_max = static_cast<uint32_t>(env_int("B200KV_STAGE_KB", 32)) << 10;
   if (g.token_bytes > stage_max || stage_max > kStageMax * 2) return B200KV_ENOTSUP;
@@ -877,6 +856,21 @@ static int engine_create_impl(const b200kv_engine_config* cfg, b200kv_pool* pool
   CU_TRY(cudaStreamCreateWithPriority(&ctx->s_d2h, cudaStreamNonBlocking, lo_pri));
   CU_TRY(cudaStreamCreateWithPriority(&ctx->s_h2d, cudaStreamNonBlocking, hi_pri));
   CU_TRY(cudaStreamCreateWithPriority(&ctx->s_scatter, cudaStreamNonBlocking, hi_pri));
+  CU_TRY(cudaEventCreateWithFlags(&ctx->fence, cudaEventDisableTiming));
+
+  // dynamic shared memory past 48 KiB, set on this device for the kernels this engine can launch; a
+  // B200KV_STAGES / B200KV_LAG pair that is not built fails at launch instead
+  if (cfg->variant != B200KV_VARIANT_LDG) {
+    for (BulkKernel k : {bulk_kernel<kStore>(ctx->S, ctx->LAG), bulk_kernel<kLoad>(ctx->S, ctx->LAG),
+                         bulk_kernel<kPull>(ctx->S, ctx->LAG)})
+      if (k) CU_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  }
+  if (cfg->format == B200KV_FMT_FP8) {
+    CU_TRY(cudaFuncSetAttribute(kv_fp8_store3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                kS3Stages * kS3MaxUnitBytes));
+    CU_TRY(cudaFuncSetAttribute(kv_fp8_store_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    CU_TRY(cudaFuncSetAttribute(kv_fp8_store_kernel<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  }
 
   CU_TRY(cudaMalloc(&ctx->d_bases, sizeof(uint64_t) * g.planes));
 
@@ -961,6 +955,7 @@ extern "C" int b200kv_engine_destroy(b200kv_ctx* ctx) {
   if (ctx->tier_base) cudaFree(ctx->tier_base);
   if (ctx->d_bases) cudaFree(ctx->d_bases);
   if (ctx->d_tmaps) cudaFree(ctx->d_tmaps);
+  if (ctx->fence) cudaEventDestroy(ctx->fence);
   for (cudaStream_t s : {ctx->s_gather, ctx->s_d2h, ctx->s_h2d, ctx->s_scatter})
     if (s) cudaStreamDestroy(s);
   delete ctx;
@@ -1065,45 +1060,26 @@ static int gather_scatter(b200kv_ctx* ctx, const int64_t* slots, int64_t n_token
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const uint32_t n_chunks = static_cast<uint32_t>((n_tokens + g.C - 1) / g.C);
 
-  std::vector<Run> runs, partial;
-  const bool fp8 = ctx->cfg.format != B200KV_FMT_RAW;   // one sorted run list for every transformed format
-  int rc = op_runs(ctx, slots, 0, n_tokens, 0, &runs, fp8 ? nullptr : &partial);
-  if (rc) return rc;
-  const size_t n_full = runs.size(), n_part = partial.size();
-  runs.insert(runs.end(), partial.begin(), partial.end());
-  TableView tv;
-  rc = table_acquire(ctx, runs.size(), n_chunks, &tv);
-  if (rc) return rc;
-  std::memcpy(tv.slot->host + tv.runs_off, runs.data(), runs.size() * sizeof(Run));
-  uint64_t* addrs = reinterpret_cast<uint64_t*>(tv.slot->host + tv.addrs_off);
-  uint32_t* offs = reinterpret_cast<uint32_t*>(tv.slot->host + tv.offs_off);
-  size_t r = 0;
+  std::vector<Span> spans(n_chunks);
+  std::vector<uint64_t> addrs(n_chunks);
   for (uint32_t c = 0; c < n_chunks; ++c) {
+    const int64_t tb = static_cast<int64_t>(c) * g.C;
+    spans[c] = {tb, std::min<int64_t>(g.C, n_tokens - tb)};
     addrs[c] = chunk_ptrs ? chunk_ptrs[c]
                           : reinterpret_cast<uint64_t>(dev_chunks) + static_cast<uint64_t>(c) * g.chunk_bytes;
-    offs[c] = static_cast<uint32_t>(r);
-    while (r < runs.size() && static_cast<uint32_t>(runs[r].b) / g.C == c) ++r;
   }
-  offs[n_chunks] = static_cast<uint32_t>(r);
-  rc = table_upload(ctx, tv, s);
+  OpTable table;
+  int rc = op_table(ctx, slots, spans, &table);
+  if (rc) return rc;
+  TableView tv;
+  rc = stage_table(ctx, table, addrs.data(), s, &tv);
   if (rc) return rc;
 
-  const int which = is_gather ? 0 : 1;
+  const int which = is_gather ? kTimeGather : kTimeScatter;
   timing_reset(ctx, which);
   rc = timing_begin(ctx, which, s);
   if (rc) return rc;
-  if (ctx->cfg.format == B200KV_FMT_FP8) {
-    std::vector<uint32_t> cn(n_chunks);
-    for (uint32_t c = 0; c < n_chunks; ++c)
-      cn[c] = static_cast<uint32_t>(std::min<int64_t>(g.C, n_tokens - static_cast<int64_t>(c) * g.C));
-    rc = is_gather ? launch_fp8_store(ctx, tv.slot->dev, tv, n_chunks, cn.data(), s)
-                   : launch_fp8_load(ctx, tv.slot->dev, tv, 0, runs.size(), s);
-  } else if (ctx->cfg.format == B200KV_FMT_Q4) {
-    rc = launch_q4(ctx, is_gather, tv.slot->dev, tv, 0, runs.size(), s);
-  } else {
-    rc = is_gather ? launch_copy_runs<kStore>(ctx, tv.slot->dev, tv, 0, n_full, n_part, s)
-                   : launch_copy_runs<kLoad>(ctx, tv.slot->dev, tv, 0, n_full, n_part, s);
-  }
+  rc = launch_op(ctx, is_gather ? kStore : kLoad, table, tv, 0, n_chunks, s);
   if (rc) return rc;
   rc = timing_end(ctx, which, s);
   if (rc) return rc;
@@ -1194,15 +1170,8 @@ static int store_impl(b200kv_ctx* ctx, const uint64_t* keys, const int32_t* chun
 
   // 0. validate every slot BEFORE touching the pool: a malformed mapping must not leave chunks
   //    reserved-but-never-committed
-  {
-    const int64_t max_slot = static_cast<int64_t>(ctx->cfg.n_blocks) * g.bs;
-    for (int32_t c = 0; c < n_chunks; ++c) {
-      if (chunk_tokens[c] <= 0 || chunk_tokens[c] > static_cast<int32_t>(g.C)) return B200KV_EINVAL;
-      const int64_t* sm = slot_mapping + static_cast<int64_t>(c) * g.C;
-      for (int32_t i = 0; i < chunk_tokens[c]; ++i)
-        if (sm[i] < 0 || sm[i] >= max_slot) return B200KV_EINVAL;
-    }
-  }
+  int rc = check_chunk_slots(ctx, slot_mapping, chunk_tokens, n_chunks);
+  if (rc) return rc;
   // 1. reserve pool slots; chunks already present (or not placeable) are skipped
   struct Todo { int32_t c; uint32_t slot; uint32_t n_tok; };
   std::vector<Todo> todo;
@@ -1210,8 +1179,7 @@ static int store_impl(b200kv_ctx* ctx, const uint64_t* keys, const int32_t* chun
   for (int32_t c = 0; c < n_chunks; ++c) {
     const uint32_t n_tok = static_cast<uint32_t>(chunk_tokens[c]);
     uint32_t slot = 0;
-    const int rc = b200kv_pool_reserve(ctx->pool, keys[c], static_cast<int32_t>(n_tok), pool_fmt(ctx),
-                                       ctx->cfg.owner, &slot);
+    rc = b200kv_pool_reserve(ctx->pool, keys[c], static_cast<int32_t>(n_tok), pool_fmt(ctx), ctx->cfg.owner, &slot);
     if (rc == B200KV_OK) { todo.push_back({c, slot, n_tok}); guard.reserved.push_back(keys[c]); }
     else if (rc != B200KV_EEXIST && rc != B200KV_ENOSPC) return rc;
   }
@@ -1223,58 +1191,35 @@ static int store_impl(b200kv_ctx* ctx, const uint64_t* keys, const int32_t* chun
   op->id = ctx->next_ticket++;
   op->pool = ctx->pool;
   CU_TRY(cudaEventCreateWithFlags(&op->done, cudaEventDisableTiming));
+  rc = stream_wait(ctx, ctx->s_gather, cs);
+  if (rc) return rc;
 
-  cudaEvent_t ev_compute;
-  CU_TRY(cudaEventCreateWithFlags(&ev_compute, cudaEventDisableTiming));
-  CU_TRY(cudaEventRecord(ev_compute, cs));
-  CU_TRY(cudaStreamWaitEvent(ctx->s_gather, ev_compute, 0));
-  CU_TRY(cudaEventDestroy(ev_compute));
-
-  timing_reset(ctx, 0);
+  timing_reset(ctx, kTimeGather);
   const size_t n_stage = ctx->n_store_slots;
   for (size_t b0 = 0; b0 < todo.size(); b0 += n_stage) {
     const size_t nb = std::min(n_stage, todo.size() - b0);
-    std::vector<Run> runs, partial;
-    std::vector<uint32_t> offs(nb + 1);
+    std::vector<Span> spans(nb);
+    for (size_t i = 0; i < nb; ++i) spans[i] = {static_cast<int64_t>(todo[b0 + i].c) * g.C, todo[b0 + i].n_tok};
+    OpTable table;
+    rc = op_table(ctx, slot_mapping, spans, &table);
+    if (rc) return rc;
     std::vector<uint64_t> addrs(nb);
-    std::vector<uint32_t> sidx(nb), batch_ntok(nb);
+    std::vector<uint32_t> sidx(nb);
     for (size_t i = 0; i < nb; ++i) {
-      const Todo& t = todo[b0 + i];
-      batch_ntok[i] = t.n_tok;
-      offs[i] = static_cast<uint32_t>(runs.size());
-      const int64_t tb = static_cast<int64_t>(t.c) * g.C;
-      // dense op-relative token index: chunk i of this batch starts at i*C
-      int rc = op_runs(ctx, slot_mapping, tb, tb + t.n_tok, tb - static_cast<int64_t>(i) * g.C, &runs,
-                       ctx->cfg.format != B200KV_FMT_RAW ? nullptr : &partial);
-      if (rc) return rc;
       sidx[i] = ctx->store_next;
       ctx->store_next = (ctx->store_next + 1) % static_cast<uint32_t>(n_stage);
       addrs[i] = reinterpret_cast<uint64_t>(ctx->d_staging) + static_cast<uint64_t>(sidx[i]) * g.chunk_bytes;
       if (ctx->stage[sidx[i]].used) CU_TRY(cudaStreamWaitEvent(ctx->s_gather, ctx->stage[sidx[i]].free_ev, 0));
     }
-    offs[nb] = static_cast<uint32_t>(runs.size());
-    const size_t n_full = runs.size(), n_part = partial.size();
-    runs.insert(runs.end(), partial.begin(), partial.end());
     TableView tv;
-    int rc = table_acquire(ctx, runs.size(), nb, &tv);
-    if (rc) return rc;
-    std::memcpy(tv.slot->host + tv.runs_off, runs.data(), runs.size() * sizeof(Run));
-    std::memcpy(tv.slot->host + tv.addrs_off, addrs.data(), nb * 8);
-    std::memcpy(tv.slot->host + tv.offs_off, offs.data(), (nb + 1) * 4);
-    rc = table_upload(ctx, tv, ctx->s_gather);
+    rc = stage_table(ctx, table, addrs.data(), ctx->s_gather, &tv);
     if (rc) return rc;
 
-    rc = timing_begin(ctx, 0, ctx->s_gather);
+    rc = timing_begin(ctx, kTimeGather, ctx->s_gather);
     if (rc) return rc;
-    if (ctx->cfg.format == B200KV_FMT_FP8) {
-      rc = launch_fp8_store(ctx, tv.slot->dev, tv, static_cast<uint32_t>(nb), batch_ntok.data(), ctx->s_gather);
-    } else if (ctx->cfg.format == B200KV_FMT_Q4) {
-      rc = launch_q4(ctx, true, tv.slot->dev, tv, 0, runs.size(), ctx->s_gather);
-    } else {
-      rc = launch_copy_runs<kStore>(ctx, tv.slot->dev, tv, 0, n_full, n_part, ctx->s_gather);
-    }
+    rc = launch_op(ctx, kStore, table, tv, 0, static_cast<uint32_t>(nb), ctx->s_gather);
     if (rc) return rc;
-    rc = timing_end(ctx, 0, ctx->s_gather);
+    rc = timing_end(ctx, kTimeGather, ctx->s_gather);
     if (rc) return rc;
     CU_TRY(cudaEventRecord(tv.slot->done_ev, ctx->s_gather));
     // the pages may be reused as soon as the gather is done: compute waits for the kernel only
@@ -1282,8 +1227,8 @@ static int store_impl(b200kv_ctx* ctx, const uint64_t* keys, const int32_t* chun
     CU_TRY(cudaStreamWaitEvent(ctx->s_d2h, tv.slot->done_ev, 0));
     for (size_t i = 0; i < nb; ++i) {
       const Todo& t = todo[b0 + i];
-      rc = copy_chunk(ctx, b200kv_pool_slot_ptr(ctx->pool, t.slot), reinterpret_cast<void*>(addrs[i]),
-                      t.n_tok, cudaMemcpyDeviceToHost, ctx->s_d2h);
+      rc = copy_chunk_planes(ctx, b200kv_pool_slot_ptr(ctx->pool, t.slot), reinterpret_cast<void*>(addrs[i]),
+                             t.n_tok, cudaMemcpyDeviceToHost, ctx->s_d2h);
       if (rc) return rc;
       CU_TRY(cudaEventRecord(ctx->stage[sidx[i]].free_ev, ctx->s_d2h));
       ctx->stage[sidx[i]].used = true;
@@ -1338,17 +1283,10 @@ static int load_impl(b200kv_ctx* ctx, const uint64_t* keys, const int32_t* chunk
   cudaStream_t cs = static_cast<cudaStream_t>(compute_stream);
   *ticket = 0;
   if (req_loaded) std::fill(req_loaded, req_loaded + n_reqs, 0);
-  {
-    const int64_t max_slot = static_cast<int64_t>(ctx->cfg.n_blocks) * g.bs;
-    for (int32_t c = 0; c < n_chunks; ++c) {   // before pinning anything
-      if (chunk_tokens[c] <= 0 || chunk_tokens[c] > static_cast<int32_t>(g.C)) return B200KV_EINVAL;
-      const int64_t* sm = slot_mapping + static_cast<int64_t>(c) * g.C;
-      for (int32_t i = 0; i < chunk_tokens[c]; ++i)
-        if (sm[i] < 0 || sm[i] >= max_slot) return B200KV_EINVAL;
-    }
-    for (int32_t r = 0; r < n_reqs; ++r)
-      if (req_first[r] > req_first[r + 1]) return B200KV_EINVAL;
-  }
+  int rc = check_chunk_slots(ctx, slot_mapping, chunk_tokens, n_chunks);   // before pinning anything
+  if (rc) return rc;
+  for (int32_t r = 0; r < n_reqs; ++r)
+    if (req_first[r] > req_first[r + 1]) return B200KV_EINVAL;
 
   struct Todo { int32_t c; uint32_t slot; uint32_t n_tok; };
   std::vector<Todo> todo;
@@ -1376,154 +1314,94 @@ static int load_impl(b200kv_ctx* ctx, const uint64_t* keys, const int32_t* chunk
   op->pool = ctx->pool;
   for (const Todo& t : todo) op->release_keys.push_back(keys[t.c]);
   // From here on every early return drops the pins and the op's events through `guard` (not every failure
-  // below is fatal: table_acquire refuses an op whose run table does not fit).
+  // below is fatal: stage_table refuses an op whose run table does not fit).
   CU_TRY(cudaEventCreateWithFlags(&op->done, cudaEventDisableTiming));
 
   const bool detached = compute_stream == B200KV_STREAM_DETACHED;
   if (!detached) {
-    cudaEvent_t ev_compute;
-    CU_TRY(cudaEventCreateWithFlags(&ev_compute, cudaEventDisableTiming));
-    CU_TRY(cudaEventRecord(ev_compute, cs));
-    CU_TRY(cudaStreamWaitEvent(ctx->s_scatter, ev_compute, 0));
-    CU_TRY(cudaEventDestroy(ev_compute));
+    rc = stream_wait(ctx, ctx->s_scatter, cs);
+    if (rc) return rc;
   }
 
-  timing_reset(ctx, 1);
+  timing_reset(ctx, kTimeScatter);
   const size_t n_stage = ctx->stage.size() - ctx->n_store_slots;
   int64_t loaded = 0;
   // Layer-wise: every chunk must own a staging slot for the whole op (the groups of all chunks are
   // interleaved); an op larger than the load half of the ring falls back to the chunk-wise path.
   const bool layerwise = layers_per_group > 0 && todo.size() <= n_stage;
-  if (layerwise) {
-    const uint32_t G = static_cast<uint32_t>(layers_per_group);
-    const uint32_t n_groups = (g.L + G - 1) / G;
-    const size_t nb = todo.size();
-    std::vector<Run> runs;
-    std::vector<uint32_t> offs(nb + 1), n_full_of(nb), sidx(nb);
-    std::vector<uint64_t> addrs(nb);
-    for (size_t i = 0; i < nb; ++i) {
-      const Todo& t = todo[i];
-      offs[i] = static_cast<uint32_t>(runs.size());
-      const int64_t tb = static_cast<int64_t>(t.c) * g.C;
-      std::vector<Run> cf, cp;
-      int rc = op_runs(ctx, slot_mapping, tb, tb + t.n_tok, tb - static_cast<int64_t>(i) * g.C, &cf,
-                       ctx->cfg.format != B200KV_FMT_RAW ? nullptr : &cp);
-      if (rc) return rc;
-      n_full_of[i] = static_cast<uint32_t>(cf.size());
-      runs.insert(runs.end(), cf.begin(), cf.end());
-      runs.insert(runs.end(), cp.begin(), cp.end());
-      sidx[i] = ctx->n_store_slots + ctx->load_next;
-      ctx->load_next = (ctx->load_next + 1) % static_cast<uint32_t>(n_stage);
-      addrs[i] = reinterpret_cast<uint64_t>(ctx->d_staging) + static_cast<uint64_t>(sidx[i]) * g.chunk_bytes;
-      StageSlot& ss = ctx->stage[sidx[i]];
-      if (ss.used) CU_TRY(cudaStreamWaitEvent(ctx->s_h2d, ss.free_ev, 0));
-      loaded += t.n_tok;
-    }
-    offs[nb] = static_cast<uint32_t>(runs.size());
-    TableView tv;
-    int rc = table_acquire(ctx, runs.size(), nb, &tv);
+  const size_t batch = layerwise ? todo.size() : n_stage;
+  for (size_t b0 = 0; b0 < todo.size(); b0 += batch) {
+    const uint32_t nb = static_cast<uint32_t>(std::min(batch, todo.size() - b0));
+    std::vector<Span> spans(nb);
+    for (uint32_t i = 0; i < nb; ++i) spans[i] = {static_cast<int64_t>(todo[b0 + i].c) * g.C, todo[b0 + i].n_tok};
+    OpTable table;
+    rc = op_table(ctx, slot_mapping, spans, &table);
     if (rc) return rc;
-    std::memcpy(tv.slot->host + tv.runs_off, runs.data(), runs.size() * sizeof(Run));
-    std::memcpy(tv.slot->host + tv.addrs_off, addrs.data(), nb * 8);
-    std::memcpy(tv.slot->host + tv.offs_off, offs.data(), (nb + 1) * 4);
-    rc = table_upload(ctx, tv, ctx->s_scatter);
-    if (rc) return rc;
-    op->layers_per_group = layers_per_group;
-    op->group_ev.resize(n_groups, nullptr);
-    cudaEvent_t landed;
-    CU_TRY(cudaEventCreateWithFlags(&landed, cudaEventDisableTiming));
-    for (uint32_t gi = 0; gi < n_groups; ++gi) {
-      const uint32_t pb = 2 * gi * G;
-      const uint32_t np = std::min<uint32_t>(2 * G, g.planes - pb);
-      for (size_t i = 0; i < nb; ++i) {
-        rc = copy_chunk_planes(ctx, reinterpret_cast<void*>(addrs[i]), b200kv_pool_slot_ptr(ctx->pool, todo[i].slot),
-                               todo[i].n_tok, pb, np, gi == 0, cudaMemcpyHostToDevice, ctx->s_h2d);
-        if (rc) return rc;
-      }
-      CU_TRY(cudaEventRecord(landed, ctx->s_h2d));           // this group of every chunk has landed
-      CU_TRY(cudaStreamWaitEvent(ctx->s_scatter, landed, 0));
-      rc = timing_begin(ctx, 1, ctx->s_scatter);
-      if (rc) return rc;
-      if (ctx->cfg.format == B200KV_FMT_FP8) {
-        rc = launch_fp8_load(ctx, tv.slot->dev, tv, 0, runs.size(), ctx->s_scatter, pb, np);
-      } else if (ctx->cfg.format == B200KV_FMT_Q4) {
-        rc = launch_q4(ctx, false, tv.slot->dev, tv, 0, runs.size(), ctx->s_scatter, pb, np);
-      } else {
-        // one launch per chunk keeps the (full, partial) run split of each chunk
-        for (size_t i = 0; i < nb && rc == B200KV_OK; ++i)
-          rc = launch_copy_runs<kLoad>(ctx, tv.slot->dev, tv, offs[i], n_full_of[i],
-                                       offs[i + 1] - offs[i] - n_full_of[i], ctx->s_scatter, nullptr, pb, np);
-      }
-      if (rc) return rc;
-      rc = timing_end(ctx, 1, ctx->s_scatter);
-      if (rc) return rc;
-      CU_TRY(cudaEventCreateWithFlags(&op->group_ev[gi], cudaEventDisableTiming));
-      CU_TRY(cudaEventRecord(op->group_ev[gi], ctx->s_scatter));
-    }
-    CU_TRY(cudaEventDestroy(landed));
-    for (size_t i = 0; i < nb; ++i) {
-      CU_TRY(cudaEventRecord(ctx->stage[sidx[i]].free_ev, ctx->s_scatter));
-      ctx->stage[sidx[i]].used = true;
-    }
-    CU_TRY(cudaEventRecord(tv.slot->done_ev, ctx->s_scatter));
-  }
-  for (size_t b0 = 0; !layerwise && b0 < todo.size(); b0 += n_stage) {
-    const size_t nb = std::min(n_stage, todo.size() - b0);
-    std::vector<Run> runs;
-    std::vector<uint32_t> offs(nb + 1);
-    std::vector<uint32_t> n_full_of(nb);
     std::vector<uint64_t> addrs(nb);
     std::vector<uint32_t> sidx(nb);
-    for (size_t i = 0; i < nb; ++i) {
-      const Todo& t = todo[b0 + i];
-      offs[i] = static_cast<uint32_t>(runs.size());
-      const int64_t tb = static_cast<int64_t>(t.c) * g.C;
-      std::vector<Run> cf, cp;  // per chunk: whole tiles first, then HND partial-tile runs
-      int rc = op_runs(ctx, slot_mapping, tb, tb + t.n_tok, tb - static_cast<int64_t>(i) * g.C, &cf,
-                       ctx->cfg.format != B200KV_FMT_RAW ? nullptr : &cp);
-      if (rc) return rc;
-      n_full_of[i] = static_cast<uint32_t>(cf.size());
-      runs.insert(runs.end(), cf.begin(), cf.end());
-      runs.insert(runs.end(), cp.begin(), cp.end());
+    for (uint32_t i = 0; i < nb; ++i) {
       sidx[i] = ctx->n_store_slots + ctx->load_next;
       ctx->load_next = (ctx->load_next + 1) % static_cast<uint32_t>(n_stage);
       addrs[i] = reinterpret_cast<uint64_t>(ctx->d_staging) + static_cast<uint64_t>(sidx[i]) * g.chunk_bytes;
+      if (layerwise && ctx->stage[sidx[i]].used) CU_TRY(cudaStreamWaitEvent(ctx->s_h2d, ctx->stage[sidx[i]].free_ev, 0));
     }
-    offs[nb] = static_cast<uint32_t>(runs.size());
     TableView tv;
-    int rc = table_acquire(ctx, runs.size(), nb, &tv);
-    if (rc) return rc;
-    std::memcpy(tv.slot->host + tv.runs_off, runs.data(), runs.size() * sizeof(Run));
-    std::memcpy(tv.slot->host + tv.addrs_off, addrs.data(), nb * 8);
-    std::memcpy(tv.slot->host + tv.offs_off, offs.data(), (nb + 1) * 4);
-    rc = table_upload(ctx, tv, ctx->s_scatter);
+    rc = stage_table(ctx, table, addrs.data(), ctx->s_scatter, &tv);
     if (rc) return rc;
 
-    for (size_t i = 0; i < nb; ++i) {
-      const Todo& t = todo[b0 + i];
-      StageSlot& ss = ctx->stage[sidx[i]];
-      if (ss.used) CU_TRY(cudaStreamWaitEvent(ctx->s_h2d, ss.free_ev, 0));
-      rc = copy_chunk(ctx, reinterpret_cast<void*>(addrs[i]), b200kv_pool_slot_ptr(ctx->pool, t.slot),
-                      t.n_tok, cudaMemcpyHostToDevice, ctx->s_h2d);
-      if (rc) return rc;
-      CU_TRY(cudaEventRecord(ss.free_ev, ctx->s_h2d));  // reused as "chunk landed" first ...
-      CU_TRY(cudaStreamWaitEvent(ctx->s_scatter, ss.free_ev, 0));
-      rc = timing_begin(ctx, 1, ctx->s_scatter);
-      if (rc) return rc;
-      const size_t r0 = offs[i], rn = offs[i + 1] - offs[i];
-      if (ctx->cfg.format == B200KV_FMT_FP8) {
-        rc = launch_fp8_load(ctx, tv.slot->dev, tv, r0, rn, ctx->s_scatter);
-      } else if (ctx->cfg.format == B200KV_FMT_Q4) {
-        rc = launch_q4(ctx, false, tv.slot->dev, tv, r0, rn, ctx->s_scatter);
-      } else {
-        rc = launch_copy_runs<kLoad>(ctx, tv.slot->dev, tv, r0, n_full_of[i], rn - n_full_of[i], ctx->s_scatter);
+    if (layerwise) {
+      const uint32_t G = static_cast<uint32_t>(layers_per_group);
+      const uint32_t n_groups = (g.L + G - 1) / G;
+      op->layers_per_group = layers_per_group;
+      op->group_ev.resize(n_groups, nullptr);
+      for (uint32_t gi = 0; gi < n_groups; ++gi) {
+        const uint32_t pb = 2 * gi * G;
+        const uint32_t np = std::min<uint32_t>(2 * G, g.planes - pb);
+        for (uint32_t i = 0; i < nb; ++i) {
+          const Todo& t = todo[b0 + i];
+          rc = copy_chunk_planes(ctx, reinterpret_cast<void*>(addrs[i]), b200kv_pool_slot_ptr(ctx->pool, t.slot),
+                                 t.n_tok, cudaMemcpyHostToDevice, ctx->s_h2d, pb, np, gi == 0);
+          if (rc) return rc;
+        }
+        rc = stream_wait(ctx, ctx->s_scatter, ctx->s_h2d);   // this group of every chunk has landed
+        if (rc) return rc;
+        rc = timing_begin(ctx, kTimeScatter, ctx->s_scatter);
+        if (rc) return rc;
+        // RAW: one launch per chunk, as on the chunk-wise path
+        const uint32_t step = ctx->cfg.format == B200KV_FMT_RAW ? 1 : nb;
+        for (uint32_t c = 0; c < nb && rc == B200KV_OK; c += step)
+          rc = launch_op(ctx, kLoad, table, tv, c, c + step, ctx->s_scatter, pb, np);
+        if (rc) return rc;
+        rc = timing_end(ctx, kTimeScatter, ctx->s_scatter);
+        if (rc) return rc;
+        CU_TRY(cudaEventCreateWithFlags(&op->group_ev[gi], cudaEventDisableTiming));
+        CU_TRY(cudaEventRecord(op->group_ev[gi], ctx->s_scatter));
       }
-      if (rc) return rc;
-      rc = timing_end(ctx, 1, ctx->s_scatter);
-      if (rc) return rc;
-      CU_TRY(cudaEventRecord(ss.free_ev, ctx->s_scatter));  // ... then as "slot drained"
-      ss.used = true;
-      loaded += t.n_tok;
+      for (uint32_t i = 0; i < nb; ++i) {
+        CU_TRY(cudaEventRecord(ctx->stage[sidx[i]].free_ev, ctx->s_scatter));
+        ctx->stage[sidx[i]].used = true;
+        loaded += todo[b0 + i].n_tok;
+      }
+    } else {
+      for (uint32_t i = 0; i < nb; ++i) {
+        const Todo& t = todo[b0 + i];
+        StageSlot& ss = ctx->stage[sidx[i]];
+        if (ss.used) CU_TRY(cudaStreamWaitEvent(ctx->s_h2d, ss.free_ev, 0));
+        rc = copy_chunk_planes(ctx, reinterpret_cast<void*>(addrs[i]), b200kv_pool_slot_ptr(ctx->pool, t.slot),
+                               t.n_tok, cudaMemcpyHostToDevice, ctx->s_h2d);
+        if (rc) return rc;
+        CU_TRY(cudaEventRecord(ss.free_ev, ctx->s_h2d));  // reused as "chunk landed" first ...
+        CU_TRY(cudaStreamWaitEvent(ctx->s_scatter, ss.free_ev, 0));
+        rc = timing_begin(ctx, kTimeScatter, ctx->s_scatter);
+        if (rc) return rc;
+        rc = launch_op(ctx, kLoad, table, tv, i, i + 1, ctx->s_scatter);
+        if (rc) return rc;
+        rc = timing_end(ctx, kTimeScatter, ctx->s_scatter);
+        if (rc) return rc;
+        CU_TRY(cudaEventRecord(ss.free_ev, ctx->s_scatter));  // ... then as "slot drained"
+        ss.used = true;
+        loaded += t.n_tok;
+      }
     }
     CU_TRY(cudaEventRecord(tv.slot->done_ev, ctx->s_scatter));
   }
@@ -1547,23 +1425,16 @@ static int load_single(b200kv_ctx* ctx, const uint64_t* keys, int32_t n_chunks, 
   if (n_chunks != static_cast<int32_t>((n_tokens + C - 1) / C)) return B200KV_EINVAL;
   if (ticket) *ticket = 0;
   if (n_loaded_tokens) *n_loaded_tokens = 0;
-  if (skip_chunks >= n_chunks) {      // nothing after the masked prefix: still validate like the general path
-    const int64_t max_slot = static_cast<int64_t>(ctx->cfg.n_blocks) * ctx->g.bs;
-    for (int64_t i = 0; i < n_tokens; ++i)
-      if (slot_mapping[i] < 0 || slot_mapping[i] >= max_slot) return B200KV_EINVAL;
-    return (ctx->pool && ctx->kv_registered && !ctx->stage.empty()) ? B200KV_OK : B200KV_EINVAL;
-  }
-  {   // slots of the masked prefix are validated too (the old single-request contract)
-    const int64_t max_slot = static_cast<int64_t>(ctx->cfg.n_blocks) * ctx->g.bs;
-    for (int64_t i = 0; i < static_cast<int64_t>(skip_chunks) * C && i < n_tokens; ++i)
-      if (slot_mapping[i] < 0 || slot_mapping[i] >= max_slot) return B200KV_EINVAL;
-  }
-  const int32_t n = n_chunks - skip_chunks;
-  std::vector<int32_t> ct(static_cast<size_t>(n));
-  for (int32_t c = 0; c < n; ++c) ct[c] = static_cast<int32_t>(std::min<int64_t>(C, n_tokens - (c + skip_chunks) * C));
-  const int32_t first[2] = {0, n};
+  std::vector<int32_t> ct(static_cast<size_t>(n_chunks));
+  for (int32_t c = 0; c < n_chunks; ++c) ct[c] = static_cast<int32_t>(std::min<int64_t>(C, n_tokens - c * C));
+  // slots of the masked prefix are validated too (the old single-request contract); load_impl checks the rest
+  const int32_t skip = std::min(skip_chunks, n_chunks);
+  const int rc_skip = check_chunk_slots(ctx, slot_mapping, ct.data(), skip);
+  if (rc_skip) return rc_skip;
+  if (skip == n_chunks) return (ctx->pool && ctx->kv_registered && !ctx->stage.empty()) ? B200KV_OK : B200KV_EINVAL;
+  const int32_t first[2] = {0, n_chunks - skip};
   int64_t loaded = 0;
-  const int rc = load_impl(ctx, keys + skip_chunks, ct.data(), n, first, 1, slot_mapping + static_cast<int64_t>(skip_chunks) * C,
+  const int rc = load_impl(ctx, keys + skip, ct.data() + skip, n_chunks - skip, first, 1, slot_mapping + skip * C,
                            compute_stream, ticket, &loaded, layers_per_group);
   if (rc == B200KV_OK && n_loaded_tokens) *n_loaded_tokens = loaded;
   return rc;
@@ -1790,48 +1661,48 @@ extern "C" int b200kv_peer_pull_async(b200kv_ctx* ctx, int32_t peer_id, const in
   cudaStream_t cs = static_cast<cudaStream_t>(compute_stream);
   *ticket = 0;
 
-  std::vector<Run> runs, partial;
+  OpTable table;
+  std::vector<Run> partial;
   int rc = build_pull_runs(src_slots, dst_slots, n_tokens, static_cast<int64_t>(peer.n_blocks) * ctx->g.bs,
                            static_cast<int64_t>(ctx->cfg.n_blocks) * ctx->g.bs, static_cast<int32_t>(ctx->g.bs),
-                           ctx->g.hnd, &runs, &partial);
+                           ctx->g.hnd, &table.runs, &partial);
   if (rc) return rc;
-  const size_t n_full = runs.size(), n_part = partial.size();
-  runs.insert(runs.end(), partial.begin(), partial.end());
+  table.full_off.push_back(static_cast<uint32_t>(table.runs.size()));
+  table.part_off.push_back(static_cast<uint32_t>(partial.size()));
+  table.runs.insert(table.runs.end(), partial.begin(), partial.end());
+  const uint64_t no_chunk = 0;   // a pull copies pages to pages: its one chunk has no buffer
   TableView tv;
-  rc = table_acquire(ctx, runs.size(), 1, &tv);
+  rc = stage_table(ctx, table, &no_chunk, ctx->s_scatter, &tv);
   if (rc) return rc;
-  std::memcpy(tv.slot->host + tv.runs_off, runs.data(), runs.size() * sizeof(Run));
 
-  std::unique_ptr<Op> op(new Op());
+  OpGuard guard(ctx, ctx->s_scatter, nullptr, nullptr, nullptr);
+  guard.op.reset(new Op());
+  Op* op = guard.op.get();
   op->id = ctx->next_ticket++;
   CU_TRY(cudaEventCreateWithFlags(&op->done, cudaEventDisableTiming));
   const bool detached = compute_stream == B200KV_STREAM_DETACHED;
   if (!detached) {
-    cudaEvent_t ev_compute;
-    CU_TRY(cudaEventCreateWithFlags(&ev_compute, cudaEventDisableTiming));
-    CU_TRY(cudaEventRecord(ev_compute, cs));
-    CU_TRY(cudaStreamWaitEvent(ctx->s_scatter, ev_compute, 0));
-    CU_TRY(cudaEventDestroy(ev_compute));
+    rc = stream_wait(ctx, ctx->s_scatter, cs);
+    if (rc) return rc;
   }
-  rc = table_upload(ctx, tv, ctx->s_scatter);
-  if (rc) return rc;
 
-  timing_reset(ctx, 2);
-  rc = timing_begin(ctx, 2, ctx->s_scatter);
+  timing_reset(ctx, kTimePull);
+  rc = timing_begin(ctx, kTimePull, ctx->s_scatter);
   if (rc) return rc;
-  rc = launch_copy_runs<kPull>(ctx, tv.slot->dev, tv, 0, n_full, n_part, ctx->s_scatter, &peer);
+  rc = launch_op(ctx, kPull, table, tv, 0, 1, ctx->s_scatter, 0, 0, &peer);
   if (rc) return rc;
-  rc = timing_end(ctx, 2, ctx->s_scatter);
+  rc = timing_end(ctx, kTimePull, ctx->s_scatter);
   if (rc) return rc;
   CU_TRY(cudaEventRecord(tv.slot->done_ev, ctx->s_scatter));
-  CU_TRY(cudaLaunchHostFunc(ctx->s_scatter, op_host_cb, op.get()));
+  CU_TRY(cudaLaunchHostFunc(ctx->s_scatter, op_host_cb, op));
   CU_TRY(cudaEventRecord(op->done, ctx->s_scatter));
   if (!detached) CU_TRY(cudaStreamWaitEvent(cs, op->done, 0));
   ++ctx->stats.n_pull_ops;
   ctx->stats.n_pulled_tokens += n_tokens;
   ctx->stats.p2p_bytes += static_cast<uint64_t>(n_tokens) * ctx->g.token_bytes * ctx->g.planes;
   *ticket = op->id;
-  ctx->ops.emplace(op->id, std::move(op));
+  ctx->ops.emplace(op->id, std::move(guard.op));
+  guard.armed = false;
   return B200KV_OK;
 }
 
@@ -1846,7 +1717,7 @@ extern "C" int b200kv_engine_get_stats(b200kv_ctx* ctx, b200kv_engine_stats* out
 }
 
 extern "C" int b200kv_last_kernel_ms(b200kv_ctx* ctx, int which, float* ms_out) {
-  if (!ctx || !ms_out || which < 0 || which > 2) return B200KV_EINVAL;
+  if (!ctx || !ms_out || which < 0 || which >= kTimingSlots) return B200KV_EINVAL;
   DeviceGuard dg(ctx->cfg.device);
   std::lock_guard<std::mutex> lk(ctx->mu);
   float total = 0.f;

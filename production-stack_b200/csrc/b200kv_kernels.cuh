@@ -759,144 +759,6 @@ __global__ void __launch_bounds__(kS3Threads, 1) kv_fp8_store3_kernel(const Fp8S
 }
 
 // ---------------------------------------------------------------------------------------------
-// FP8 store, two-pass variant (B200KV_FP8_2PASS=1; experimental): same grid, cluster and output as
-// kv_fp8_store_kernel, but no shared-memory staging.  Pass 1 streams the CTA's window straight from
-// the pages into the per-head absmax; after the cluster exchange pass 2 reads the same bytes again —
-// an L2 hit, the slab was touched microseconds ago — quantises and stores.  HBM is still read once;
-// without the 64 KiB of smem per CTA residency is bounded by registers/threads, not by smem.
-// Per token the kernel keeps one source address in smem (NHD: the token's row; HND: row 0 of head 0
-// of its tile position), filled by warp 0 from the run list.
-// ---------------------------------------------------------------------------------------------
-constexpr int kMaxWindow = 64;  // tokens per CTA window (C / kCluster)
-constexpr int kBatch = 8;       // 16-byte loads a thread keeps in flight
-
-__global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(256, 4)
-    kv_fp8_store2_kernel(const Fp8StoreParams p) {
-  __shared__ uint64_t s_src[kMaxWindow];
-  __shared__ uint32_t s_absmax[kMaxHeads];
-  __shared__ uint32_t s_all[kMaxHeads];
-  __shared__ float s_inv[kMaxHeads];
-
-  const uint32_t rank = cluster_ctarank();
-  const uint32_t slab = blockIdx.x / kCluster;
-  const uint32_t c = slab / p.n_planes;
-  const uint32_t plane = slab - c * p.n_planes;
-  const uint32_t W = p.chunk_tokens / kCluster;
-  const uint32_t tb = p.paged.token_bytes;
-  const uint32_t bs = p.paged.block_tokens;
-  const uint32_t win_lo = c * p.chunk_tokens + rank * W;
-  uint32_t n_valid = 0;
-  // tokens of this chunk = end of its last run (runs are sorted by b): a batch of several requests may hold
-  // partial chunks anywhere, not only at its end
-  uint32_t chunk_hi = c * p.chunk_tokens;
-  {
-    const uint32_t rr0 = p.chunk_run_off[c], rr1 = p.chunk_run_off[c + 1];
-    if (rr1 > rr0) chunk_hi = static_cast<uint32_t>(p.runs[rr1 - 1].b + p.runs[rr1 - 1].n);
-  }
-  if (win_lo < chunk_hi) n_valid = min(W, chunk_hi - win_lo);
-  if (win_lo + n_valid > chunk_hi) n_valid = chunk_hi > win_lo ? chunk_hi - win_lo : 0;
-
-  if (threadIdx.x < kMaxHeads) {
-    s_absmax[threadIdx.x] = 0;
-    s_all[threadIdx.x] = 0;
-  }
-  if (threadIdx.x < 32) {
-    const uint32_t r0 = p.chunk_run_off[c], r1 = p.chunk_run_off[c + 1];
-    for (uint32_t r = r0 + threadIdx.x; r < r1; r += 32) {
-      const Run run = p.runs[r];
-      const int32_t lo = max(run.b, static_cast<int32_t>(win_lo));
-      const int32_t hi = min(run.b + run.n, static_cast<int32_t>(win_lo + n_valid));
-      for (int32_t t = lo; t < hi; ++t) {
-        const uint32_t slot = static_cast<uint32_t>(run.a + (t - run.b));
-        s_src[t - static_cast<int32_t>(win_lo)] =
-            p.hnd ? paged_addr_hnd(p.paged, plane, slot, 0, p.head_bytes) : paged_addr(p.paged, plane, slot);
-      }
-    }
-  }
-  __syncthreads();
-  cluster_arrive_release();  // split barrier #1: s_all is zeroed everywhere before any push
-
-  const uint32_t vpt = tb >> 4;            // 16-byte vectors per token
-  const uint32_t rv = p.head_bytes >> 4;   // ... per (token, head) row
-  const uint32_t head_stride = p.hnd ? bs * p.head_bytes : p.head_bytes;  // bytes between heads of one token
-  // thread -> fixed column (head h, vector cc) ; token groups share the columns when vpt < 256
-  const uint32_t groups = vpt < 256 ? 256 / vpt : 1;
-  const uint32_t grp = threadIdx.x / vpt;
-  const bool active = grp < groups;
-  const uint32_t col0 = threadIdx.x - grp * vpt;
-  const uint32_t col_step = groups == 1 ? 256u : vpt;
-
-  // ---- pass 1: absmax straight from the pages ----
-  if (active) {
-    for (uint32_t col = col0; col < vpt; col += col_step) {
-      const uint32_t h = col / rv, cc = col - h * rv;
-      const uint64_t off = static_cast<uint64_t>(h) * head_stride + static_cast<uint64_t>(cc) * 16;
-      uint32_t acc = 0;
-      for (uint32_t t0 = grp; t0 < n_valid; t0 += groups * kBatch) {
-        uint4 v[kBatch];  // all loads of a batch are issued before the first one is consumed
-#pragma unroll
-        for (int j = 0; j < kBatch; ++j) {
-          const uint32_t t = t0 + j * groups;
-          v[j] = t < n_valid ? ld_nc_v4(reinterpret_cast<const void*>(s_src[t] + off)) : make_uint4(0, 0, 0, 0);
-        }
-#pragma unroll
-        for (int j = 0; j < kBatch; ++j)
-          acc = absmax_u16x2(absmax_u16x2(absmax_u16x2(absmax_u16x2(acc, v[j].x), v[j].y), v[j].z), v[j].w);
-      }
-      const uint32_t m = max(acc & 0xffffu, acc >> 16);
-      if (m) atomicMax(&s_absmax[h], m);
-    }
-  }
-  __syncthreads();
-  cluster_wait_acquire();  // #1
-  if (threadIdx.x < p.n_heads) {
-    const uint32_t mine = s_absmax[threadIdx.x];
-#pragma unroll
-    for (uint32_t r = 0; r < kCluster; ++r) red_dsmem_max_u32(&s_all[threadIdx.x], r, mine);
-  }
-  cluster_arrive_release();  // #2: all pushes have landed; nothing remote is touched afterwards
-  cluster_wait_acquire();
-  if (threadIdx.x < p.n_heads) {
-    const uint32_t m = s_all[threadIdx.x];
-    const float amax = __uint_as_float(m << 16);
-    s_inv[threadIdx.x] = (m == 0) ? 1.0f : __fdiv_rn(448.0f, amax);
-    if (rank == 0) {
-      float* scales = reinterpret_cast<float*>(p.chunk_addrs[c] + p.scales_off);
-      scales[plane * p.n_heads + threadIdx.x] = (m == 0) ? 1.0f : __fdiv_rn(amax, 448.0f);
-    }
-  }
-  __syncthreads();
-
-  // ---- pass 2: the same bytes again (L2), quantise, store ----
-  uint8_t* out = reinterpret_cast<uint8_t*>(p.chunk_addrs[c] + static_cast<uint64_t>(plane) * p.slab_q_bytes +
-                                            static_cast<uint64_t>(rank * W) * (tb >> 1));
-  if (active) {
-    for (uint32_t col = col0; col < vpt; col += col_step) {
-      const uint32_t h = col / rv, cc = col - h * rv;
-      const uint64_t off = static_cast<uint64_t>(h) * head_stride + static_cast<uint64_t>(cc) * 16;
-      const float inv = s_inv[h];
-      for (uint32_t t0 = grp; t0 < n_valid; t0 += groups * kBatch) {
-        uint4 v[kBatch];
-#pragma unroll
-        for (int j = 0; j < kBatch; ++j) {
-          const uint32_t t = t0 + j * groups;
-          v[j] = t < n_valid ? ld_nc_v4(reinterpret_cast<const void*>(s_src[t] + off)) : make_uint4(0, 0, 0, 0);
-        }
-#pragma unroll
-        for (int j = 0; j < kBatch; ++j) {
-          const uint32_t t = t0 + j * groups;
-          if (t >= n_valid) break;
-          // NHD chunk: token-major; HND chunk: tiles verbatim, ((tile*H + h)*bs + row)*rv + cc
-          const size_t idx = p.hnd ? (static_cast<size_t>((t / bs) * p.n_heads + h) * bs + (t % bs)) * rv + cc
-                                   : static_cast<size_t>(t) * vpt + col;
-          st_na_v2(out + idx * 8, quant8(v[j], inv));
-        }
-      }
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
 // FP8 load: one CTA per (run, plane) unit; e4m3 * scale -> bf16 (RN) into the pages.
 // ---------------------------------------------------------------------------------------------
 struct Fp8LoadParams {

@@ -107,4 +107,58 @@ inline int build_pull_runs(const int64_t* src, const int64_t* dst, int64_t n_tok
   return B200KV_OK;
 }
 
+// The run table of one op: the full runs of every chunk, chunk by chunk, then the partial runs of every
+// chunk, chunk by chunk.  Chunk i's full runs are runs[full_off[i], full_off[i+1]) and its partial runs
+// runs[n_full() + part_off[i], n_full() + part_off[i+1]).
+struct OpTable {
+  std::vector<Run> runs;
+  std::vector<uint32_t> full_off{0};
+  std::vector<uint32_t> part_off{0};
+  uint32_t n_chunks() const { return static_cast<uint32_t>(full_off.size() - 1); }
+  uint32_t n_full() const { return full_off.back(); }
+};
+
+// Chunk i of a table holds slots[tok_begin, tok_begin + n_tok) and starts at op-relative index i*C.
+struct Span {
+  int64_t tok_begin;
+  int64_t n_tok;
+};
+
+// The table of an op over `spans`.  `split` (RAW) keeps HND partial-tile runs apart; without it every
+// run is a full run.  Returns B200KV_EINVAL if a slot lies outside [0, max_slot).
+inline int build_op_table(const int64_t* slots, const Span* spans, size_t n_spans, int64_t max_slot, int32_t bs,
+                          int32_t C, bool split, bool hnd, OpTable* t) {
+  *t = OpTable();
+  std::vector<Run> partial;
+  for (size_t i = 0; i < n_spans; ++i) {
+    const int64_t tb = spans[i].tok_begin;
+    const int rc = build_runs(slots, tb, tb + spans[i].n_tok, tb - static_cast<int64_t>(i) * C, max_slot, bs, C,
+                              hnd, &t->runs, split ? &partial : nullptr);
+    if (rc) return rc;
+    t->full_off.push_back(static_cast<uint32_t>(t->runs.size()));
+    t->part_off.push_back(static_cast<uint32_t>(partial.size()));
+  }
+  t->runs.insert(t->runs.end(), partial.begin(), partial.end());
+  return B200KV_OK;
+}
+
+// Byte layout of a table as the kernels read it: the runs, the chunk addresses, then full_off (the FP8
+// store kernels' per-chunk run offsets), each rounded up to 16 bytes.  A table over kTableBytes is refused.
+constexpr size_t kTableBytes = 1u << 20;
+
+struct TableLayout {
+  size_t runs_off, addrs_off, offs_off, bytes;
+};
+
+inline int table_layout(size_t n_runs, size_t n_chunks, TableLayout* l) {
+  const size_t runs_bytes = (n_runs * sizeof(Run) + 15) / 16 * 16;
+  const size_t addrs_bytes = (n_chunks * 8 + 15) / 16 * 16;
+  const size_t offs_bytes = ((n_chunks + 1) * 4 + 15) / 16 * 16;
+  l->runs_off = 0;
+  l->addrs_off = runs_bytes;
+  l->offs_off = runs_bytes + addrs_bytes;
+  l->bytes = runs_bytes + addrs_bytes + offs_bytes;
+  return l->bytes > kTableBytes ? B200KV_EINVAL : B200KV_OK;
+}
+
 }  // namespace b200kv

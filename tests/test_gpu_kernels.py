@@ -564,39 +564,6 @@ def test_layerwise_retrieve_matches_oracle(group, fmt, layout):
 
 
 # ------------------------------------------------------------------------------------------------
-# B200KV_FP8_2PASS=1: the smem-free two-pass FP8 store kernel must produce the same chunk, byte for
-# byte (codes and scales), as the default kernel, which the tests above hold against the oracle.
-# ------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("hnd", [False, True])
-@pytest.mark.parametrize("n_tok", [1, 15, 16, 17, 40, 255, 256, 257, 700, 1024])
-def test_fp8_two_pass_store_equals_default_kernel(monkeypatch, hnd, n_tok):
-    need_gpu()
-    p = SMALL
-    rng = np.random.default_rng(9000 + n_tok)
-    host = mk_host_layers(rng, p["L"], p["NB"], p["bs"], p["H"], p["D"])
-    dev = to_dev_hnd(host) if hnd else to_dev(host)
-    geom = KVGeometry(p["L"], p["H"], p["D"], p["NB"], p["bs"], p["C"], 2, 2 * p["bs"] * p["H"] * p["D"] * 2 if hnd else 0,
-                      FMT_FP8, b200kv._lib.LAYOUT_HND if hnd else b200kv._lib.LAYOUT_NHD)
-    if n_tok == 40:      # token-granular: every token in another block
-        sm = rng.permutation(p["NB"] * p["bs"])[:n_tok].astype(np.int64)
-    else:
-        sm = ko.slot_mapping_from_blocks(rng.permutation(p["NB"])[: (n_tok + p["bs"] - 1) // p["bs"]], p["bs"], n_tok)
-    n_chunks = (n_tok + p["C"] - 1) // p["C"]
-    out = []
-    monkeypatch.setenv("B200KV_FP8_STORE", "1")       # compare the two cluster kernels (the default is kernel 3)
-    for two_pass in ("0", "1"):
-        monkeypatch.setenv("B200KV_FP8_2PASS", two_pass)
-        eng = KVEngine(geom, None, 0, staging_bytes=0)
-        eng.register_kv_caches(dev)
-        buf = torch.zeros(n_chunks * geom.chunk_bytes, dtype=torch.uint8, device="cuda:0")
-        eng.gather(sm, buf.data_ptr())
-        torch.cuda.synchronize()
-        out.append(buf.cpu().numpy())
-        eng.close()
-    assert np.array_equal(out[0], out[1])
-
-
-# ------------------------------------------------------------------------------------------------
 # The default FP8 store is the persistent warp-specialised kernel (kv_fp8_store3_kernel; TMA tensor maps on
 # NHD pages, bulk copies on HND pages); ops it does not take (token-granular mappings) run the cluster
 # kernel.  Both must produce the same chunk, byte for byte, and the tests above hold whichever runs

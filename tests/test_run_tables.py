@@ -36,6 +36,29 @@ extern "C" int op_runs(const int64_t* slots, int64_t tok_begin, int64_t tok_end,
   return rc;
 }
 
+extern "C" int op_table(const int64_t* slots, const int64_t* spans, int64_t n_spans, int64_t max_slot, int32_t bs,
+                        int32_t C, int split, int hnd, Run* runs, int64_t* n_runs, uint32_t* full_off,
+                        uint32_t* part_off) {
+  std::vector<b200kv::Span> sp;
+  for (int64_t i = 0; i < n_spans; ++i) sp.push_back({spans[2 * i], spans[2 * i + 1]});
+  b200kv::OpTable t;
+  const int rc = b200kv::build_op_table(slots, sp.data(), sp.size(), max_slot, bs, C, split != 0, hnd != 0, &t);
+  out(t.runs, runs, n_runs);
+  for (size_t i = 0; i < t.full_off.size(); ++i) full_off[i] = t.full_off[i];
+  for (size_t i = 0; i < t.part_off.size(); ++i) part_off[i] = t.part_off[i];
+  return rc;
+}
+
+extern "C" int table_layout(int64_t n_runs, int64_t n_chunks, uint64_t* l) {
+  b200kv::TableLayout t;
+  const int rc = b200kv::table_layout(static_cast<size_t>(n_runs), static_cast<size_t>(n_chunks), &t);
+  l[0] = t.runs_off;
+  l[1] = t.addrs_off;
+  l[2] = t.offs_off;
+  l[3] = t.bytes;
+  return rc;
+}
+
 extern "C" int pull_runs(const int64_t* src, const int64_t* dst, int64_t n, int64_t max_src, int64_t max_dst,
                          int32_t bs, int hnd, Run* full, int64_t* n_full, Run* part, int64_t* n_part) {
   std::vector<Run> f, p;
@@ -279,3 +302,94 @@ def test_bench_shape_gives_one_run_per_block(lib):
     assert all(r[2] == 16 for r in full)
     assert [r[1] for r in full] == list(range(0, n, 16))
     assert [r[0] for r in full] == [int(slots[i]) for i in range(0, n, 16)]
+
+
+def build_table(lib, slots, spans, max_slot, bs, c, split, hnd):
+    slots = np.ascontiguousarray(slots, np.int64)
+    sp = np.ascontiguousarray(np.asarray(spans, np.int64).reshape(-1, 2))
+    n_tok = int(sp[:, 1].sum())
+    runs = np.zeros((max(n_tok, 1), 3), np.int32)
+    full_off, part_off = np.zeros(len(sp) + 1, np.uint32), np.zeros(len(sp) + 1, np.uint32)
+    n = C.c_int64(-1)
+    rc = lib.op_table(_p(slots), _p(sp), C.c_int64(len(sp)), C.c_int64(max_slot), C.c_int32(bs), C.c_int32(c),
+                      C.c_int(split), C.c_int(hnd), _p(runs), C.byref(n), _p(full_off), _p(part_off))
+    if rc:
+        return rc, None, None, None
+    return rc, [tuple(r) for r in runs[:n.value]], list(map(int, full_off)), list(map(int, part_off))
+
+
+def ref_table(slots, spans, max_slot, bs, c, split, hnd):
+    """Each span's runs from the per-token rule, chunk i indexed from i*C, regrouped: every chunk's full
+    runs, chunk by chunk, then every chunk's partial runs."""
+    full, part, full_off, part_off = [], [], [0], [0]
+    for i, (tb, n) in enumerate(spans):
+        rc, f, p = ref(slots, tb, tb + n, tb - i * c, max_slot, bs, c, hnd, split)
+        if rc:
+            return rc, None, None, None
+        full += f
+        part += p
+        full_off.append(len(full))
+        part_off.append(len(part))
+    return 0, full + part, full_off, part_off
+
+
+@pytest.mark.parametrize("hnd", [False, True])
+@pytest.mark.parametrize("bs,c", GEOMS)
+def test_op_table_regroups_the_runs_of_ragged_spans(lib, bs, c, hnd):
+    """Store / load batches: any chunks of the op, each 1..C tokens, laid out as chunks 0, 1, ... of one table."""
+    rng = np.random.default_rng(500 + bs * 100 + c + hnd)
+    nb = 64
+    for _ in range(60):
+        n_op = int(rng.integers(1, 9))                      # chunks of the op, C slots apart
+        slots = random_map(rng, n_op * c, nb, bs)
+        picked = sorted(rng.choice(n_op, int(rng.integers(1, n_op + 1)), replace=False))
+        spans = [(int(k) * c, int(rng.integers(1, c + 1))) for k in picked]
+        for split in (True, False):
+            want = ref_table(slots, spans, nb * bs, bs, c, split, hnd)
+            assert want[0] == 0
+            assert build_table(lib, slots, spans, nb * bs, bs, c, split, hnd) == want
+    slots[0] = nb * bs                                       # a slot out of range refuses the table
+    assert build_table(lib, slots, [(0, 1)], nb * bs, bs, c, True, hnd)[0] == EINVAL
+
+
+@pytest.mark.parametrize("hnd", [False, True])
+@pytest.mark.parametrize("bs,c", GEOMS)
+def test_gather_spans_give_the_whole_op_runs(lib, bs, c, hnd):
+    """Gather / scatter: spans [k*C, min((k+1)*C, n)) give exactly the runs of one build over the whole op, and,
+    for the FP8 / Q4 table (no split), full_off is where each chunk's runs start by their op-relative index."""
+    rng = np.random.default_rng(900 + bs * 100 + c + hnd)
+    nb = 64
+    for _ in range(60):
+        n = int(rng.integers(1, 6 * c))
+        slots = random_map(rng, n, nb, bs)
+        spans = [(k, min(c, n - k)) for k in range(0, n, c)]
+        for split in (True, False):
+            rc, full, part = build(lib, slots, 0, n, 0, nb * bs, bs, c, hnd, split)
+            got = build_table(lib, slots, spans, nb * bs, bs, c, split, hnd)
+            assert rc == 0 and got[0] == 0 and got[1] == full + part
+            if not split:
+                offs, r = [], 0
+                for k in range(len(spans)):
+                    offs.append(r)
+                    while r < len(full) and full[r][1] // c == k:
+                        r += 1
+                offs.append(r)
+                assert got[2] == offs
+
+
+def test_table_layout_and_its_cap(lib):
+    def layout(n_runs, n_chunks):
+        out = np.zeros(4, np.uint64)
+        rc = lib.table_layout(C.c_int64(n_runs), C.c_int64(n_chunks), _p(out))
+        return rc, list(map(int, out))
+
+    def up16(x):
+        return (x + 15) // 16 * 16
+
+    for n_runs in (0, 1, 2, 5, 2048, 87378):
+        for n_chunks in (1, 2, 3, 7, 128, 1000):
+            runs, addrs, offs = up16(12 * n_runs), up16(8 * n_chunks), up16(4 * (n_chunks + 1))
+            total = runs + addrs + offs
+            assert layout(n_runs, n_chunks) == ((0 if total <= 1 << 20 else EINVAL), [0, runs, runs + addrs, total])
+    assert layout(87378, 1) == (0, [0, 1048544, 1048560, 1 << 20])      # one chunk: exactly 1 MiB
+    assert layout(87379, 1)[0] == EINVAL
