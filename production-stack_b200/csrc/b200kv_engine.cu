@@ -196,6 +196,16 @@ int make_geometry(const b200kv_engine_config* c, Geometry* g) {
   return B200KV_OK;
 }
 
+// The geometry kv_fp8_store3_kernel needs: a (chunk, head) unit of bf16 fits one consumer group's registers, a
+// row is a whole number of 16-byte vectors that divides the group, one block's rows of a head fill whole 128-byte
+// lines, a chunk has at most 256 blocks, and (HND) one step of the group's tokens is whole tiles.
+bool fp8_store3_fits(const Geometry& g) {
+  const uint32_t rv = g.row_bytes >> 4;
+  return g.elem == 2 && static_cast<uint64_t>(g.C) * g.row_bytes <= kS3MaxUnitBytes && (g.row_bytes & 15) == 0 &&
+         rv != 0 && kS3GroupThreads % rv == 0 && (static_cast<uint64_t>(g.bs) * g.row_bytes) % 128 == 0 &&
+         g.C / g.bs <= 32 * 8 && !(g.hnd && (kS3GroupThreads / rv) % g.bs != 0);
+}
+
 }  // namespace
 
 struct b200kv_ctx {
@@ -238,8 +248,8 @@ struct b200kv_ctx {
 
   // bulk-kernel launch shape
   int S = 2, LAG = 1, ctas_per_sm = 1;  // B200KV_STAGES / B200KV_LAG / B200KV_CTAS_PER_SM (tools/sweep.py)
-  int fp8_threads = 256;                // B200KV_FP8_THREADS: CTA width of the FP8 store kernel
-  int fp8_store_ver = 3;                // B200KV_FP8_STORE: 3 = persistent warp-specialised kernel (default), 1 = cluster kernel
+  bool fp8_store3 = false;              // FP8 stores may take kv_fp8_store3_kernel: its geometry fits, and
+                                        // B200KV_FP8_STORE (3 = that kernel, the default; 1 = cluster kernel) allows it
   void* d_tmaps = nullptr;              // one CUtensorMap per plane (NHD pages: strided [bs][D] boxes for the FP8 store)
   std::string tmap_status = "not built";
   uint32_t piece_tokens = 0, pieces = 0, stage_bytes = 0;
@@ -362,7 +372,7 @@ int launched(b200kv_ctx* ctx) {
   return B200KV_OK;
 }
 
-typedef void (*BulkKernel)(CopyParams, uint32_t);
+typedef void (*BulkKernel)(KernelArgs, uint32_t);
 
 // the bulk kernel built for a B200KV_STAGES / B200KV_LAG pair; null for a pair that is not built
 template <int MODE>
@@ -380,25 +390,6 @@ BulkKernel bulk_kernel(int S, int LAG) {
   }
 }
 
-template <int MODE>
-int launch_copy(b200kv_ctx* ctx, const CopyParams& p, cudaStream_t s) {
-  if (ctx->cfg.variant == B200KV_VARIANT_LDG) {
-    uint32_t grid = static_cast<uint32_t>(ctx->sm_count * 8);
-    grid = std::min(grid, p.total_units);
-    if (grid == 0) return B200KV_OK;
-    kv_ldg_copy_kernel<MODE><<<grid, 256, 0, s>>>(p);
-    return launched(ctx);
-  }
-  const BulkKernel kernel = bulk_kernel<MODE>(ctx->S, ctx->LAG);
-  if (!kernel) return B200KV_EINVAL;
-  const size_t smem = 256 + static_cast<size_t>(ctx->S) * ctx->stage_bytes;
-  uint32_t grid = static_cast<uint32_t>(ctx->sm_count * ctx->ctas_per_sm);
-  grid = std::min(grid, p.total_units);
-  if (grid == 0) return B200KV_OK;
-  kernel<<<grid, 32, smem, s>>>(p, ctx->stage_bytes);
-  return launched(ctx);
-}
-
 // format tag recorded with a chunk: a pool shared by engines of different tile order or codec
 // never hands one engine's bytes to another
 uint32_t pool_fmt(const b200kv_ctx* ctx) {
@@ -414,176 +405,98 @@ PagedSide local_side(const b200kv_ctx* ctx) {
   return s;
 }
 
-// Full runs [f0, f0 + nf) of the table go to the bulk (or LDG) kernel, HND partial-tile runs [p0, p0 + np)
+// The parameter block of a launch over runs [run_begin, ...) of the staged table `tv`, planes [plane_begin,
+// plane_begin + n_planes) (n_planes == 0: every plane).  `peer` non-null is the pull source.  The launcher sets
+// total_units.
+KernelArgs kernel_args(const b200kv_ctx* ctx, const TableView& tv, size_t run_begin, uint32_t plane_begin,
+                       uint32_t n_planes, const Peer* peer = nullptr) {
+  const Geometry& g = ctx->g;
+  KernelArgs a{};
+  a.paged = local_side(ctx);
+  a.peer = a.paged;
+  if (peer) {
+    a.peer.bases = peer->d_bases;
+    a.peer.block_stride = peer->block_stride;
+  }
+  a.chunk.chunk_addrs = tv.chunk_addrs;
+  a.chunk.slab_bytes = g.slab_bytes;
+  a.chunk.scales_off = g.scales_off;
+  a.chunk.chunk_tokens = g.C;
+  a.chunk.token_bytes = g.fmt_token_bytes;
+  a.runs = tv.runs + run_begin;
+  a.chunk_run_off = tv.full_off;
+  a.plane_begin = plane_begin;
+  a.n_planes = n_planes ? n_planes : g.planes;
+  a.n_heads = g.H;
+  a.row_bytes = g.row_bytes;
+  a.hnd = g.hnd ? 1u : 0u;
+  a.pieces = ctx->pieces;
+  a.piece_tokens = ctx->piece_tokens;
+  return a;
+}
+
+// RAW: full runs [f0, f0 + nf) of the table go to the bulk (or LDG) kernel, HND partial-tile runs [p0, p0 + np)
 // to kv_hnd_partial_kernel.  `peer` non-null selects the pull source.
 template <int MODE>
 int launch_copy_runs(b200kv_ctx* ctx, const TableView& tv, size_t f0, size_t nf, size_t p0, size_t np,
                      cudaStream_t s, const Peer* peer, uint32_t plane_begin, uint32_t n_planes) {
-  CopyParams p{};
-  p.paged = local_side(ctx);
-  p.peer = p.paged;
-  if (peer) {
-    p.peer.bases = peer->d_bases;
-    p.peer.block_stride = peer->block_stride;
-  }
-  p.chunk.chunk_addrs = tv.chunk_addrs;
-  p.chunk.slab_bytes = ctx->g.slab_bytes;
-  p.chunk.chunk_tokens = ctx->g.C;
-  p.chunk.token_bytes = ctx->g.fmt_token_bytes;
-  p.runs = tv.runs + f0;
-  p.n_runs = static_cast<uint32_t>(nf);
-  p.n_planes = n_planes ? n_planes : ctx->g.planes;
-  p.plane_begin = plane_begin;
-  p.pieces = ctx->pieces;
-  p.piece_tokens = ctx->piece_tokens;
-  p.total_units = p.n_runs * p.n_planes * p.pieces;
   if (nf) {
-    const int rc = launch_copy<MODE>(ctx, p, s);
-    if (rc) return rc;
-  }
-  if (np == 0) return B200KV_OK;
-  HndParams h{};
-  h.paged = p.paged;
-  h.peer = p.peer;
-  h.chunk = p.chunk;
-  h.runs = tv.runs + p0;
-  h.n_runs = static_cast<uint32_t>(np);
-  h.n_planes = p.n_planes;
-  h.plane_begin = p.plane_begin;
-  h.n_heads = ctx->g.H;
-  h.row_bytes = ctx->g.row_bytes;
-  h.total_units = h.n_runs * h.n_planes * h.n_heads;
-  const uint32_t grid = std::min<uint32_t>(h.total_units, static_cast<uint32_t>(ctx->sm_count) * 16u);
-  kv_hnd_partial_kernel<MODE><<<grid, 128, 0, s>>>(h);
-  return launched(ctx);
-}
-
-// Persistent FP8 store (kv_fp8_store3_kernel) when every chunk of the batch is a sequence of whole, block-aligned
-// runs (the last possibly short).  Returns 1 if it launched, 0 if the batch is not eligible, < 0 on error.
-int try_launch_fp8_store3(b200kv_ctx* ctx, const OpTable& t, const TableView& tv, cudaStream_t s) {
-  const Geometry& g = ctx->g;
-  const uint32_t n_chunks = t.n_chunks();
-  const uint32_t head_bytes = g.D * 2, rv = head_bytes >> 4;
-  const uint64_t unit_bytes = static_cast<uint64_t>(g.C) * head_bytes;
-  if (ctx->fp8_store_ver != 3 || g.elem != 2 || unit_bytes > kS3MaxUnitBytes || (head_bytes & 15) || rv == 0 ||
-      (kS3GroupThreads % rv) != 0 || (static_cast<uint64_t>(g.bs) * head_bytes) % 128 != 0 || g.C / g.bs > 32 * 8 ||
-      (g.hnd && (kS3GroupThreads / rv) % g.bs != 0))
-    return 0;
-  const bool use_tmap = !g.hnd || env_int("B200KV_FP8_TMAP_HND", 0);
-  if (use_tmap && (!ctx->d_tmaps || ctx->tmap_status != "ok")) return 0;
-  const Run* runs = t.runs.data();
-  const uint32_t* offs = t.full_off.data();
-  for (uint32_t c = 0; c < n_chunks; ++c) {
-    const uint32_t base = c * g.C;
-    uint32_t n_valid = 0;   // the chunk's tokens: its runs cover them
-    for (uint32_t r = offs[c]; r < offs[c + 1]; ++r) n_valid += static_cast<uint32_t>(runs[r].n);
-    if (n_valid == 0 || n_valid > g.C) return 0;
-    const uint32_t nb = (n_valid + g.bs - 1) / g.bs;
-    if (offs[c + 1] - offs[c] != nb) return 0;
-    for (uint32_t j = 0; j < nb; ++j) {
-      const Run& r = runs[offs[c] + j];
-      if (r.b != static_cast<int32_t>(base + j * g.bs) || (static_cast<uint32_t>(r.a) % g.bs) != 0 ||
-          static_cast<uint32_t>(r.n) != std::min<uint32_t>(g.bs, n_valid - j * g.bs))
-        return 0;
+    KernelArgs a = kernel_args(ctx, tv, f0, plane_begin, n_planes, peer);
+    a.total_units = static_cast<uint32_t>(nf) * a.n_planes * a.pieces;
+    const bool ldg = ctx->cfg.variant == B200KV_VARIANT_LDG;
+    const BulkKernel kernel = ldg ? nullptr : bulk_kernel<MODE>(ctx->S, ctx->LAG);
+    if (!ldg && !kernel) return B200KV_EINVAL;
+    const uint32_t grid = std::min(static_cast<uint32_t>(ctx->sm_count * (ldg ? 8 : ctx->ctas_per_sm)), a.total_units);
+    if (grid) {
+      if (ldg) kv_ldg_copy_kernel<MODE><<<grid, 256, 0, s>>>(a);
+      else kernel<<<grid, 32, 256 + static_cast<size_t>(ctx->S) * ctx->stage_bytes, s>>>(a, ctx->stage_bytes);
+      const int rc = launched(ctx);
+      if (rc) return rc;
     }
   }
-  Fp8Store3Params p{};
-  p.paged = local_side(ctx);
-  p.runs = tv.runs;
-  p.chunk_run_off = tv.full_off;
-  p.chunk_addrs = tv.chunk_addrs;
-  p.tmaps = use_tmap ? ctx->d_tmaps : nullptr;
-  p.n_chunks = n_chunks;
-  p.n_planes = g.planes;
-  p.chunk_tokens = g.C;
-  p.n_tokens = 0;   // unused: a chunk's token count comes from its runs
-  p.n_heads = g.H;
-  p.head_bytes = head_bytes;
-  p.slab_q_bytes = g.slab_bytes;
-  p.scales_off = g.scales_off;
-  p.hnd = g.hnd ? 1u : 0u;
-  p.total_units = n_chunks * g.planes * g.H;
-  const size_t smem = static_cast<size_t>(kS3Stages) * unit_bytes;
-  const uint32_t grid = std::min<uint32_t>(p.total_units, static_cast<uint32_t>(ctx->sm_count));
-  if (grid == 0) return 1;
-  kv_fp8_store3_kernel<<<grid, kS3Threads, smem, s>>>(p);
-  const int rc = launched(ctx);
-  return rc ? rc : 1;
+  if (np == 0) return B200KV_OK;
+  KernelArgs a = kernel_args(ctx, tv, p0, plane_begin, n_planes, peer);
+  a.total_units = static_cast<uint32_t>(np) * a.n_planes * a.n_heads;
+  const uint32_t grid = std::min<uint32_t>(a.total_units, static_cast<uint32_t>(ctx->sm_count) * 16u);
+  kv_hnd_partial_kernel<MODE><<<grid, 128, 0, s>>>(a);
+  return launched(ctx);
 }
 
-// Every chunk of the table; chunks of several requests may be partial anywhere.
+// FP8 store of every chunk of the table; chunks of several requests may be partial anywhere.  The persistent
+// kernel takes the table when the engine allows it (fp8_store3) and every chunk is whole, block-aligned runs; the
+// cluster kernel takes every other table.
 int launch_fp8_store(b200kv_ctx* ctx, const OpTable& t, const TableView& tv, cudaStream_t s) {
-  {
-    const int rc3 = try_launch_fp8_store3(ctx, t, tv, s);
-    if (rc3 != 0) return rc3 < 0 ? rc3 : B200KV_OK;
+  const Geometry& g = ctx->g;
+  KernelArgs a = kernel_args(ctx, tv, 0, 0, 0);
+  if (ctx->fp8_store3 && (g.hnd || ctx->tmap_status == "ok") && whole_block_chunks(t, g.bs, g.C)) {
+    a.total_units = t.n_chunks() * g.planes * g.H;
+    const size_t smem = static_cast<size_t>(kS3Stages) * g.C * g.row_bytes;
+    const uint32_t grid = std::min<uint32_t>(a.total_units, static_cast<uint32_t>(ctx->sm_count));
+    if (grid == 0) return B200KV_OK;
+    kv_fp8_store3_kernel<<<grid, kS3Threads, smem, s>>>(a, g.hnd ? nullptr : ctx->d_tmaps);
+    return launched(ctx);
   }
-  const uint32_t n_chunks = t.n_chunks();
-  Fp8StoreParams p{};   // n_tokens stays 0: unused (see above)
-  p.paged = local_side(ctx);
-  p.runs = tv.runs;
-  p.chunk_run_off = tv.full_off;
-  p.chunk_addrs = tv.chunk_addrs;
-  p.n_chunks = n_chunks;
-  p.n_planes = ctx->g.planes;
-  p.chunk_tokens = ctx->g.C;
-  p.n_heads = ctx->g.H;
-  p.head_bytes = ctx->g.D * 2;
-  p.slab_q_bytes = ctx->g.slab_bytes;
-  p.scales_off = ctx->g.scales_off;
-  p.hnd = ctx->g.hnd ? 1u : 0u;
-  const size_t smem = static_cast<size_t>(ctx->g.C / kCluster) * ctx->g.token_bytes;
+  const size_t smem = static_cast<size_t>(g.C / kCluster) * g.token_bytes;
   if (smem > 200 * 1024) return B200KV_ENOTSUP;
-  const uint32_t grid = kCluster * n_chunks * ctx->g.planes;
+  const uint32_t grid = kCluster * t.n_chunks() * g.planes;
   if (grid == 0) return B200KV_OK;
-  if (ctx->fp8_threads == 512) kv_fp8_store_kernel<512><<<grid, 512, smem, s>>>(p);
-  else kv_fp8_store_kernel<256><<<grid, 256, smem, s>>>(p);
+  kv_fp8_store_kernel<<<grid, kFp8Threads, smem, s>>>(a);
   return launched(ctx);
 }
 
-int launch_fp8_load(b200kv_ctx* ctx, const TableView& tv, size_t run_begin, size_t n_runs, cudaStream_t s,
-                    uint32_t plane_begin, uint32_t n_planes) {
-  Fp8LoadParams p{};
-  p.paged = local_side(ctx);
-  p.runs = tv.runs + run_begin;
-  p.chunk_addrs = tv.chunk_addrs;
-  p.n_runs = static_cast<uint32_t>(n_runs);
-  p.n_planes = n_planes ? n_planes : ctx->g.planes;
-  p.plane_begin = plane_begin;
-  p.chunk_tokens = ctx->g.C;
-  p.n_heads = ctx->g.H;
-  p.head_bytes = ctx->g.D * 2;
-  p.slab_q_bytes = ctx->g.slab_bytes;
-  p.scales_off = ctx->g.scales_off;
-  p.hnd = ctx->g.hnd ? 1u : 0u;
-  p.total_units = p.n_runs * p.n_planes;
-  const size_t smem = static_cast<size_t>(ctx->g.bs) * ctx->g.fmt_token_bytes;
+// FP8 load, Q4 store and Q4 load of runs [f0, f0 + nf): one unit per (run, plane).
+int launch_per_run(b200kv_ctx* ctx, CopyMode mode, const TableView& tv, size_t f0, size_t nf, cudaStream_t s,
+                   uint32_t plane_begin, uint32_t n_planes) {
+  const bool fp8 = ctx->cfg.format == B200KV_FMT_FP8;
+  const size_t smem = fp8 ? static_cast<size_t>(ctx->g.bs) * ctx->g.fmt_token_bytes : 0;
   if (smem > 48 * 1024) return B200KV_ENOTSUP;
-  uint32_t grid = std::min<uint32_t>(p.total_units, static_cast<uint32_t>(ctx->sm_count) * 8u);
+  KernelArgs a = kernel_args(ctx, tv, f0, plane_begin, n_planes);
+  a.total_units = static_cast<uint32_t>(nf) * a.n_planes;
+  const uint32_t grid = std::min<uint32_t>(a.total_units, static_cast<uint32_t>(ctx->sm_count) * 8u);
   if (grid == 0) return B200KV_OK;
-  kv_fp8_load_kernel<<<grid, kFp8Threads, smem, s>>>(p);
-  return launched(ctx);
-}
-
-int launch_q4(b200kv_ctx* ctx, bool store, const TableView& tv, size_t run_begin, size_t n_runs, cudaStream_t s,
-              uint32_t plane_begin, uint32_t n_planes) {
-  Q4Params p{};
-  p.paged = local_side(ctx);
-  p.runs = tv.runs + run_begin;
-  p.chunk_addrs = tv.chunk_addrs;
-  p.n_runs = static_cast<uint32_t>(n_runs);
-  p.n_planes = n_planes ? n_planes : ctx->g.planes;
-  p.plane_begin = plane_begin;
-  p.chunk_tokens = ctx->g.C;
-  p.n_heads = ctx->g.H;
-  p.head_bytes = ctx->g.D * 2;
-  p.slab_bytes = ctx->g.slab_bytes;
-  p.rec_bytes = ctx->g.fmt_token_bytes;
-  p.hnd = ctx->g.hnd ? 1u : 0u;
-  p.total_units = p.n_runs * p.n_planes;
-  const uint32_t grid = std::min<uint32_t>(p.total_units, static_cast<uint32_t>(ctx->sm_count) * 8u);
-  if (grid == 0) return B200KV_OK;
-  if (store) kv_q4_store_kernel<<<grid, 256, 0, s>>>(p);
-  else kv_q4_load_kernel<<<grid, 256, 0, s>>>(p);
+  if (fp8) kv_fp8_load_kernel<<<grid, kFp8Threads, smem, s>>>(a);
+  else if (mode == kStore) kv_q4_store_kernel<<<grid, 256, 0, s>>>(a);
+  else kv_q4_load_kernel<<<grid, 256, 0, s>>>(a);
   return launched(ctx);
 }
 
@@ -594,9 +507,8 @@ int launch_op(b200kv_ctx* ctx, CopyMode mode, const OpTable& t, const TableView&
               cudaStream_t s, uint32_t pb = 0, uint32_t np = 0, const Peer* peer = nullptr) {
   const size_t f0 = t.full_off[c0], nf = t.full_off[c1] - f0;
   const int fmt = mode == kPull ? B200KV_FMT_RAW : ctx->cfg.format;
-  if (fmt == B200KV_FMT_FP8)
-    return mode == kStore ? launch_fp8_store(ctx, t, tv, s) : launch_fp8_load(ctx, tv, f0, nf, s, pb, np);
-  if (fmt == B200KV_FMT_Q4) return launch_q4(ctx, mode == kStore, tv, f0, nf, s, pb, np);
+  if (fmt == B200KV_FMT_FP8 && mode == kStore) return launch_fp8_store(ctx, t, tv, s);
+  if (fmt != B200KV_FMT_RAW) return launch_per_run(ctx, mode, tv, f0, nf, s, pb, np);
   const size_t p0 = t.n_full() + t.part_off[c0], n_part = t.part_off[c1] - t.part_off[c0];
   switch (mode) {
     case kStore: return launch_copy_runs<kStore>(ctx, tv, f0, nf, p0, n_part, s, peer, pb, np);
@@ -841,8 +753,7 @@ static int engine_create_impl(const b200kv_engine_config* cfg, b200kv_pool* pool
   ctx->S = cfg->stages > 0 ? cfg->stages : env_int("B200KV_STAGES", 2);
   ctx->LAG = env_int("B200KV_LAG", ctx->S / 2);
   ctx->ctas_per_sm = cfg->ctas_per_sm > 0 ? cfg->ctas_per_sm : env_int("B200KV_CTAS_PER_SM", 1);
-  ctx->fp8_threads = env_int("B200KV_FP8_THREADS", 256) == 512 ? 512 : 256;
-  ctx->fp8_store_ver = env_int("B200KV_FP8_STORE", 3);
+  ctx->fp8_store3 = cfg->format == B200KV_FMT_FP8 && env_int("B200KV_FP8_STORE", 3) == 3 && fp8_store3_fits(g);
   const uint32_t stage_max = static_cast<uint32_t>(env_int("B200KV_STAGE_KB", 32)) << 10;
   if (g.token_bytes > stage_max || stage_max > kStageMax * 2) return B200KV_ENOTSUP;
   ctx->piece_tokens = std::min<uint32_t>(g.bs, stage_max / g.token_bytes);
@@ -868,8 +779,7 @@ static int engine_create_impl(const b200kv_engine_config* cfg, b200kv_pool* pool
   if (cfg->format == B200KV_FMT_FP8) {
     CU_TRY(cudaFuncSetAttribute(kv_fp8_store3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 kS3Stages * kS3MaxUnitBytes));
-    CU_TRY(cudaFuncSetAttribute(kv_fp8_store_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    CU_TRY(cudaFuncSetAttribute(kv_fp8_store_kernel<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    CU_TRY(cudaFuncSetAttribute(kv_fp8_store_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   }
 
   CU_TRY(cudaMalloc(&ctx->d_bases, sizeof(uint64_t) * g.planes));
@@ -962,14 +872,14 @@ extern "C" int b200kv_engine_destroy(b200kv_ctx* ctx) {
   return B200KV_OK;
 }
 
-// One 4-D tensor map per plane over the paged cache, so that TMA can fetch "the bs rows of head h in block b"
-// — a [bs][D] box whose rows are a token apart — as ONE copy (SASS UTMALDG).  Dimensions are ordered by
-// ascending stride: NHD pages {D, H, bs, NB} (box {D, 1, bs, 1}), HND pages {D, bs, H, NB} (box {D, bs, 1, 1});
-// the box always lands as [bs][D] in shared memory.  Failure is not fatal: the FP8 store then runs its
-// cluster kernel.
+// One 4-D tensor map per plane over NHD pages, so that TMA can fetch "the bs rows of head h in block b" — a
+// [bs][D] box whose rows are a token apart — as ONE copy (SASS UTMALDG).  Dimensions are ordered by ascending
+// stride: {D, H, bs, NB}, box {D, 1, bs, 1}, which lands as [bs][D] in shared memory.  HND pages need no map:
+// those rows are contiguous and a plain bulk copy fetches them.  Failure is not fatal: the FP8 store then runs
+// its cluster kernel.
 static void build_tensor_maps(b200kv_ctx* ctx, const std::vector<uint64_t>& bases) {
   const Geometry& g = ctx->g;
-  if (ctx->cfg.format != B200KV_FMT_FP8 || g.elem != 2) { ctx->tmap_status = "not needed"; return; }
+  if (ctx->cfg.format != B200KV_FMT_FP8 || g.elem != 2 || g.hnd) { ctx->tmap_status = "not needed"; return; }
   typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -985,15 +895,8 @@ static void build_tensor_maps(b200kv_ctx* ctx, const std::vector<uint64_t>& base
   std::vector<CUtensorMap> maps(g.planes);
   const cuuint64_t row = static_cast<cuuint64_t>(g.D) * g.elem, tok = g.token_bytes, blk = ctx->cfg.block_stride_bytes;
   for (uint32_t pl = 0; pl < g.planes; ++pl) {
-    cuuint64_t dims[4], strides[3];
-    cuuint32_t box[4], estr[4] = {1, 1, 1, 1};
-    dims[0] = g.D;
-    dims[3] = ctx->cfg.n_blocks;
-    if (g.hnd) { dims[1] = g.bs; dims[2] = g.H; strides[0] = row; strides[1] = row * g.bs; box[1] = g.bs; box[2] = 1; }
-    else       { dims[1] = g.H; dims[2] = g.bs; strides[0] = row; strides[1] = tok;        box[1] = 1; box[2] = g.bs; }
-    strides[2] = blk;
-    box[0] = g.D;
-    box[3] = 1;
+    const cuuint64_t dims[4] = {g.D, g.H, g.bs, ctx->cfg.n_blocks}, strides[3] = {row, tok, blk};
+    const cuuint32_t box[4] = {g.D, 1, g.bs, 1}, estr[4] = {1, 1, 1, 1};
     const CUresult r = reinterpret_cast<EncodeFn>(fn)(&maps[pl], CU_TENSOR_MAP_DATA_TYPE_UINT16, 4,
                                                       reinterpret_cast<void*>(bases[pl]), dims, strides, box, estr,
                                                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,

@@ -10,18 +10,27 @@
 // that matter are coalescing, enough bytes in flight per SM to cover DRAM latency, and a grid
 // that is a multiple of the SM count (132 on H100).
 //
-//   kv_bulk_copy_kernel  RAW store / load / peer pull.  One elected thread per CTA drives the
-//                        TMA engine: cp.async.bulk global->smem (mbarrier complete_tx) into an
-//                        S-stage ring, then cp.async.bulk smem->global (bulk_group).  No
-//                        registers touch the payload.  Persistent grid.
-//   kv_ldg_copy_kernel   same contract with 128-bit ld.global.nc / st.global (A/B variant).
-//   kv_fp8_store_kernel  cluster of 8 CTAs per (chunk, layer, K/V) slab: warp 0 bulk-loads the CTA's 32
-//                        tokens into smem (one run per lane), per-head absmax in registers -> smem,
-//                        every CTA pushes its maxima into all 8 CTAs' smem with DSMEM atomics
-//                        (red.shared::cluster.max) between a split cluster barrier (arrive early,
-//                        wait late) and one full one, quantise to e4m3 from smem, coalesced stores.
-//                        HBM is read exactly once.  NHD and HND tiles.
-//   kv_fp8_load_kernel   bulk-load e4m3 piece -> dequantise -> 16-byte stores into the pages.
+//   kv_bulk_copy_kernel    RAW store / load / peer pull.  One elected thread per CTA drives the
+//                          TMA engine: cp.async.bulk global->smem (mbarrier complete_tx) into an
+//                          S-stage ring, then cp.async.bulk smem->global (bulk_group).  No
+//                          registers touch the payload.  Persistent grid.
+//   kv_ldg_copy_kernel     same contract with 128-bit ld.global.nc / st.global (A/B variant).
+//   kv_hnd_partial_kernel  RAW runs that cover part of an HND tile, moved one (run, plane, head) row
+//                          range at a time.
+//   kv_fp8_store3_kernel   FP8 store of block-structured ops (the default): persistent, warp-specialised;
+//                          a TMA producer warp feeds two consumer groups, one (chunk, plane, head) unit
+//                          at a time.
+//   kv_fp8_store_kernel    FP8 store of every other op: cluster of 8 CTAs per (chunk, layer, K/V) slab;
+//                          warp 0 bulk-loads the CTA's tokens into smem (one run per lane), per-head
+//                          absmax in registers -> smem, every CTA pushes its maxima into all 8 CTAs'
+//                          smem with DSMEM atomics (red.shared::cluster.max) between a split cluster
+//                          barrier (arrive early, wait late) and one full one, quantise to e4m3 from
+//                          smem, coalesced stores.  HBM is read exactly once.  NHD and HND tiles.
+//   kv_fp8_load_kernel     bulk-load e4m3 piece -> dequantise -> 16-byte stores into the pages.
+//   kv_q4_store_kernel /   group-wise 4-bit chunks: one 16-byte vector per thread, a group is a quad
+//   kv_q4_load_kernel      of lanes.
+//
+// Every kernel takes one KernelArgs, filled by kernel_args() in b200kv_engine.cu.
 #pragma once
 
 #include <cuda_bf16.h>
@@ -42,23 +51,32 @@ struct PagedSide {
 
 struct ChunkSide {
   const uint64_t* chunk_addrs;  // device array [n_chunks]: where chunk c of this op lives
-  uint64_t slab_bytes;          // C * token_bytes(format): one (layer, K/V) slab
+  uint64_t slab_bytes;          // C * token_bytes: one (layer, K/V) slab
   uint32_t chunk_tokens;
-  uint32_t token_bytes;         // bytes per token per slab in this format (RAW: 2048, FP8: 1024)
+  uint32_t token_bytes;         // bytes per token per slab in this format: RAW H*D*elem, FP8 H*D, Q4 one record
+  uint64_t scales_off;          // FP8: byte offset of the (planes, H) fp32 scales inside a chunk
 };
 
-struct CopyParams {
-  PagedSide paged;        // local pages (store src / load dst / pull dst)
-  PagedSide peer;         // pull src (peer mapping); unused otherwise
+// The one parameter block of every kernel.  A field a kernel does not read is still filled.  It must stay within
+// 128 bytes: nvcc keeps a larger by-value kernel parameter in memory and reads every field through its address,
+// which costs registers (kv_q4_store_kernel: 39 -> 47).  The order of the 32-bit fields keeps the bulk copy
+// kernel's parameter loads, and so its code, as they were.
+struct KernelArgs {
+  PagedSide paged;                // local pages (store src / load dst / pull dst)
+  PagedSide peer;                 // pull src (peer mapping)
   ChunkSide chunk;
   const Run* runs;
-  uint32_t n_runs;
-  uint32_t n_planes;      // planes covered by this launch (2*L, or one layer group of it)
-  uint32_t plane_begin;   // first plane of the launch (layer-wise loads walk the planes in groups)
-  uint32_t pieces;        // pieces per run = ceil(block_tokens / piece_tokens)
-  uint32_t piece_tokens;  // tokens per piece (piece bytes <= stage bytes)
-  uint32_t total_units;   // n_runs * n_planes * pieces
+  const uint32_t* chunk_run_off;  // FP8 stores: [n_chunks+1] run range of each chunk
+  uint32_t n_heads;
+  uint32_t n_planes;              // planes covered by this launch (2*L, or one layer group of it)
+  uint32_t plane_begin;           // first plane of the launch (layer-wise loads walk the planes in groups)
+  uint32_t pieces;                // bulk copy: pieces per run = ceil(block_tokens / piece_tokens)
+  uint32_t piece_tokens;          // bulk copy: tokens per piece (piece bytes <= stage bytes)
+  uint32_t total_units;           // units of work of the launch; each kernel says what its unit is
+  uint32_t row_bytes;             // D * elem: one (token, head) row (D*2 for FP8 / Q4, which take bf16 only)
+  uint32_t hnd;                   // pages hold [H][block_tokens][D] tiles
 };
+static_assert(sizeof(KernelArgs) <= 128, "KernelArgs must stay within 128 bytes (see above)");
 
 enum CopyMode { kStore = 0, kLoad = 1, kPull = 2 };
 
@@ -176,11 +194,56 @@ __device__ __forceinline__ uint64_t paged_addr(const PagedSide& s, uint32_t plan
   return __ldg(s.bases + plane) + static_cast<uint64_t>(blk) * s.block_stride +
          static_cast<uint64_t>(off) * s.token_bytes;
 }
-__device__ __forceinline__ uint64_t chunk_addr(const ChunkSide& s, uint32_t plane, uint32_t tok) {
+// HND tiles: row `off` of head h inside the slot's block
+__device__ __forceinline__ uint64_t paged_addr_hnd(const PagedSide& s, uint32_t plane, uint32_t slot,
+                                                   uint32_t h, uint32_t row_bytes) {
+  const uint32_t blk = slot / s.block_tokens;
+  const uint32_t off = slot - blk * s.block_tokens;
+  return __ldg(s.bases + plane) + static_cast<uint64_t>(blk) * s.block_stride +
+         static_cast<uint64_t>(h) * s.block_tokens * row_bytes + static_cast<uint64_t>(off) * row_bytes;
+}
+
+// an op-relative token index as (chunk c, token t inside chunk c)
+struct ChunkPos {
+  uint32_t c, t;
+};
+__device__ __forceinline__ ChunkPos chunk_pos(const ChunkSide& s, uint32_t tok) {
   const uint32_t c = tok / s.chunk_tokens;
-  const uint32_t t = tok - c * s.chunk_tokens;
-  return __ldg(s.chunk_addrs + c) + static_cast<uint64_t>(plane) * s.slab_bytes +
-         static_cast<uint64_t>(t) * s.token_bytes;
+  return {c, tok - c * s.chunk_tokens};
+}
+
+__device__ __forceinline__ uint64_t chunk_addr(const ChunkSide& s, uint32_t plane, uint32_t tok) {
+  const ChunkPos cp = chunk_pos(s, tok);
+  return __ldg(s.chunk_addrs + cp.c) + static_cast<uint64_t>(plane) * s.slab_bytes +
+         static_cast<uint64_t>(cp.t) * s.token_bytes;
+}
+// HND: the chunk stores the tiles verbatim
+__device__ __forceinline__ uint64_t chunk_addr_hnd(const ChunkSide& s, uint32_t plane, uint32_t tok,
+                                                   uint32_t h, uint32_t block_tokens, uint32_t row_bytes) {
+  const ChunkPos cp = chunk_pos(s, tok);
+  const uint32_t tile = cp.t / block_tokens;
+  const uint32_t off = cp.t - tile * block_tokens;
+  return __ldg(s.chunk_addrs + cp.c) + static_cast<uint64_t>(plane) * s.slab_bytes +
+         static_cast<uint64_t>(tile) * block_tokens * s.token_bytes +
+         static_cast<uint64_t>(h) * block_tokens * row_bytes + static_cast<uint64_t>(off) * row_bytes;
+}
+
+// Source and destination of a RAW copy by direction, `off` tokens into the run: a store reads the pages at slot
+// run.a and writes the chunk at token run.b, a load the other way round, a pull reads the peer's pages at slot
+// run.a and writes the local pages at slot run.b.  paged(side, slot) and chunk(tok) give one side's address.
+template <int MODE, class PagedAt, class ChunkAt>
+__device__ __forceinline__ void copy_ends(const KernelArgs& p, const Run& run, int32_t off, PagedAt paged,
+                                          ChunkAt chunk, uint64_t* src, uint64_t* dst) {
+  if (MODE == kStore) {
+    *src = paged(p.paged, static_cast<uint32_t>(run.a + off));
+    *dst = chunk(static_cast<uint32_t>(run.b + off));
+  } else if (MODE == kLoad) {
+    *src = chunk(static_cast<uint32_t>(run.b + off));
+    *dst = paged(p.paged, static_cast<uint32_t>(run.a + off));
+  } else {
+    *src = paged(p.peer, static_cast<uint32_t>(run.a + off));
+    *dst = paged(p.paged, static_cast<uint32_t>(run.b + off));
+  }
 }
 
 struct Unit {
@@ -189,7 +252,7 @@ struct Unit {
 };
 
 template <int MODE>
-__device__ __forceinline__ Unit decode_unit(const CopyParams& p, uint32_t u) {
+__device__ __forceinline__ Unit decode_unit(const KernelArgs& p, uint32_t u) {
   // plane fastest: consecutive units of one CTA stride across planes of the same run.
   const uint32_t plane = p.plane_begin + u % p.n_planes;
   const uint32_t t = u / p.n_planes;
@@ -201,16 +264,10 @@ __device__ __forceinline__ Unit decode_unit(const CopyParams& p, uint32_t u) {
   n = n < 0 ? 0 : (n > static_cast<int32_t>(p.piece_tokens) ? static_cast<int32_t>(p.piece_tokens) : n);
   Unit out;
   out.bytes = static_cast<uint32_t>(n) * p.paged.token_bytes;
-  if (MODE == kStore) {
-    out.src = paged_addr(p.paged, plane, static_cast<uint32_t>(run.a + off));
-    out.dst = chunk_addr(p.chunk, plane, static_cast<uint32_t>(run.b + off));
-  } else if (MODE == kLoad) {
-    out.src = chunk_addr(p.chunk, plane, static_cast<uint32_t>(run.b + off));
-    out.dst = paged_addr(p.paged, plane, static_cast<uint32_t>(run.a + off));
-  } else {
-    out.src = paged_addr(p.peer, plane, static_cast<uint32_t>(run.a + off));
-    out.dst = paged_addr(p.paged, plane, static_cast<uint32_t>(run.b + off));
-  }
+  copy_ends<MODE>(
+      p, run, off,
+      [&](const PagedSide& s, uint32_t slot) { return paged_addr(s, plane, slot); },
+      [&](uint32_t tok) { return chunk_addr(p.chunk, plane, tok); }, &out.src, &out.dst);
   return out;
 }
 
@@ -221,8 +278,9 @@ __device__ __forceinline__ Unit decode_unit(const CopyParams& p, uint32_t u) {
 //                 (A) wait for unit j-LAG's bytes, issue its bulk store, commit one group.
 // Loads in flight per CTA: LAG; stores in flight: S-LAG.
 // ---------------------------------------------------------------------------------------------
+// A unit is one piece of one run in one plane: total_units = n_runs * n_planes * pieces.
 template <int MODE, int S, int LAG>
-__global__ void __launch_bounds__(32) kv_bulk_copy_kernel(const CopyParams p, uint32_t stage_bytes) {
+__global__ void __launch_bounds__(32) kv_bulk_copy_kernel(const KernelArgs p, uint32_t stage_bytes) {
   static_assert(LAG >= 1 && LAG < S, "need 1 <= LAG < S");
   extern __shared__ __align__(128) uint8_t smem[];
   uint64_t* full = reinterpret_cast<uint64_t*>(smem);               // S mbarriers
@@ -267,7 +325,7 @@ __global__ void __launch_bounds__(32) kv_bulk_copy_kernel(const CopyParams p, ui
 // RAW path, LSU variant: a CTA copies one unit at a time with 128-bit loads, 4 in flight/thread.
 // ---------------------------------------------------------------------------------------------
 template <int MODE>
-__global__ void __launch_bounds__(256) kv_ldg_copy_kernel(const CopyParams p) {
+__global__ void __launch_bounds__(256) kv_ldg_copy_kernel(const KernelArgs p) {
   for (uint32_t ui = blockIdx.x; ui < p.total_units; ui += gridDim.x) {
     const Unit u = decode_unit<MODE>(p, ui);
     const uint4* __restrict__ src = reinterpret_cast<const uint4*>(u.src);
@@ -290,54 +348,22 @@ __global__ void __launch_bounds__(256) kv_ldg_copy_kernel(const CopyParams p) {
 // HND tiles ([H][block_tokens][D] inside a block).  A whole-block run is one contiguous tile and
 // goes through the kernels above unchanged (the chunk stores tiles verbatim).  Runs that cover
 // only part of a tile — the ragged tail of a request, or token-granular mappings — are moved
-// per head by this kernel: one unit = (run, plane, head) = n * D * elem contiguous bytes.
+// per head by this kernel: one unit = (run, plane, head) = n * D * elem contiguous bytes, so
+// total_units = n_runs * n_planes * n_heads.
 // ---------------------------------------------------------------------------------------------
-struct HndParams {
-  PagedSide paged, peer;
-  ChunkSide chunk;       // chunk.token_bytes = H*D*elem; a tile = block_tokens * token_bytes
-  const Run* runs;
-  uint32_t n_runs, n_planes, n_heads;
-  uint32_t plane_begin;
-  uint32_t row_bytes;    // D * elem: one (token, head) row
-  uint32_t total_units;  // n_runs * n_planes * n_heads
-};
-
-__device__ __forceinline__ uint64_t paged_addr_hnd(const PagedSide& s, uint32_t plane, uint32_t slot,
-                                                   uint32_t h, uint32_t row_bytes) {
-  const uint32_t blk = slot / s.block_tokens;
-  const uint32_t off = slot - blk * s.block_tokens;
-  return __ldg(s.bases + plane) + static_cast<uint64_t>(blk) * s.block_stride +
-         static_cast<uint64_t>(h) * s.block_tokens * row_bytes + static_cast<uint64_t>(off) * row_bytes;
-}
-__device__ __forceinline__ uint64_t chunk_addr_hnd(const ChunkSide& s, uint32_t plane, uint32_t tok,
-                                                   uint32_t h, uint32_t block_tokens, uint32_t row_bytes) {
-  const uint32_t c = tok / s.chunk_tokens;
-  const uint32_t t = tok - c * s.chunk_tokens;
-  const uint32_t tile = t / block_tokens;
-  const uint32_t off = t - tile * block_tokens;
-  return __ldg(s.chunk_addrs + c) + static_cast<uint64_t>(plane) * s.slab_bytes +
-         static_cast<uint64_t>(tile) * block_tokens * s.token_bytes +
-         static_cast<uint64_t>(h) * block_tokens * row_bytes + static_cast<uint64_t>(off) * row_bytes;
-}
-
 template <int MODE>
-__global__ void __launch_bounds__(128) kv_hnd_partial_kernel(const HndParams p) {
+__global__ void __launch_bounds__(128) kv_hnd_partial_kernel(const KernelArgs p) {
   for (uint32_t ui = blockIdx.x; ui < p.total_units; ui += gridDim.x) {
     const uint32_t h = ui % p.n_heads;
     const uint32_t t = ui / p.n_heads;
     const uint32_t plane = p.plane_begin + t % p.n_planes;
     const Run run = p.runs[t / p.n_planes];
     uint64_t src, dst;
-    if (MODE == kStore) {
-      src = paged_addr_hnd(p.paged, plane, static_cast<uint32_t>(run.a), h, p.row_bytes);
-      dst = chunk_addr_hnd(p.chunk, plane, static_cast<uint32_t>(run.b), h, p.paged.block_tokens, p.row_bytes);
-    } else if (MODE == kLoad) {
-      src = chunk_addr_hnd(p.chunk, plane, static_cast<uint32_t>(run.b), h, p.paged.block_tokens, p.row_bytes);
-      dst = paged_addr_hnd(p.paged, plane, static_cast<uint32_t>(run.a), h, p.row_bytes);
-    } else {
-      src = paged_addr_hnd(p.peer, plane, static_cast<uint32_t>(run.a), h, p.row_bytes);
-      dst = paged_addr_hnd(p.paged, plane, static_cast<uint32_t>(run.b), h, p.row_bytes);
-    }
+    copy_ends<MODE>(
+        p, run, 0,
+        [&](const PagedSide& s, uint32_t slot) { return paged_addr_hnd(s, plane, slot, h, p.row_bytes); },
+        [&](uint32_t tok) { return chunk_addr_hnd(p.chunk, plane, tok, h, p.paged.block_tokens, p.row_bytes); },
+        &src, &dst);
     const uint32_t nvec = (static_cast<uint32_t>(run.n) * p.row_bytes) >> 4;
     for (uint32_t i = threadIdx.x; i < nvec; i += 128)
       st_na_v4(reinterpret_cast<uint4*>(dst) + i, ld_nc_v4(reinterpret_cast<const uint4*>(src) + i));
@@ -351,20 +377,6 @@ __global__ void __launch_bounds__(128) kv_hnd_partial_kernel(const HndParams p) 
 constexpr int kCluster = 8;
 constexpr int kFp8Threads = 256;
 constexpr int kMaxHeads = 64;
-
-struct Fp8StoreParams {
-  PagedSide paged;
-  const Run* runs;                // sorted by b
-  const uint32_t* chunk_run_off;  // [n_chunks+1] run range of each chunk
-  const uint64_t* chunk_addrs;    // [n_chunks] destination of each chunk
-  uint32_t n_chunks, n_planes;
-  uint32_t chunk_tokens;          // C
-  uint32_t n_tokens;              // op length
-  uint32_t n_heads, head_bytes;   // H, D*2
-  uint64_t slab_q_bytes;          // C * H * D   (e4m3 bytes per slab)
-  uint64_t scales_off;            // byte offset of the (planes, H) fp32 scales inside a chunk
-  uint32_t hnd;                   // tiles are [H][block_tokens][D]; the packed chunk mirrors them
-};
 
 __device__ __forceinline__ uint32_t absmax_u16x2(uint32_t acc, uint32_t w) {
   return __vmaxu2(acc, w & 0x7fff7fffu);
@@ -387,9 +399,8 @@ __device__ __forceinline__ uint2 quant8(const uint4& v, float inv) {
   return make_uint2(o[0], o[1]);
 }
 
-template <int kThreads>
-__global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kThreads)
-    kv_fp8_store_kernel(const Fp8StoreParams p) {
+__global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kFp8Threads)
+    kv_fp8_store_kernel(const KernelArgs p) {
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ __align__(8) uint64_t bar;
   __shared__ uint32_t s_absmax[kMaxHeads];  // this CTA's |x| max per head (bf16 bits: integer order == magnitude)
@@ -400,13 +411,13 @@ __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kThreads)
   const uint32_t slab = blockIdx.x / kCluster;
   const uint32_t c = slab / p.n_planes;
   const uint32_t plane = slab - c * p.n_planes;
-  const uint32_t W = p.chunk_tokens / kCluster;
+  const uint32_t W = p.chunk.chunk_tokens / kCluster;
   const uint32_t tb = p.paged.token_bytes;
-  const uint32_t win_lo = c * p.chunk_tokens + rank * W;  // op-relative token index
+  const uint32_t win_lo = c * p.chunk.chunk_tokens + rank * W;  // op-relative token index
   uint32_t n_valid = 0;
   // tokens of this chunk = end of its last run (runs are sorted by b): a batch of several requests may hold
   // partial chunks anywhere, not only at its end
-  uint32_t chunk_hi = c * p.chunk_tokens;
+  uint32_t chunk_hi = c * p.chunk.chunk_tokens;
   {
     const uint32_t rr0 = p.chunk_run_off[c], rr1 = p.chunk_run_off[c + 1];
     if (rr1 > rr0) chunk_hi = static_cast<uint32_t>(p.runs[rr1 - 1].b + p.runs[rr1 - 1].n);
@@ -444,7 +455,7 @@ __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kThreads)
         mine += n * tb;
       } else {
         // partial HND tile: one piece per head (runs never cross a tile on either side)
-        const uint32_t row = p.head_bytes;  // D*2
+        const uint32_t row = p.row_bytes;  // D*2
         uint8_t* tile = smem + static_cast<size_t>(rel / bs) * bs * tb + static_cast<size_t>(rel % bs) * row;
         for (uint32_t h = 0; h < p.n_heads; ++h) {
           bulk_g2s(tile + static_cast<size_t>(h) * bs * row,
@@ -464,7 +475,7 @@ __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kThreads)
 
   const uint32_t vpt = tb >> 4;  // 16-byte vectors per token
   // HND window = W/bs whole tiles [H][bs][D]: vector idx = ((tile*H + h)*bs + row)*rv + c.
-  const uint32_t rv = p.head_bytes >> 4;                 // 16-byte vectors per (token, head) row
+  const uint32_t rv = p.row_bytes >> 4;                 // 16-byte vectors per (token, head) row
   const uint32_t tile_rows = p.paged.block_tokens * rv;  // vectors per (tile, head)
   const uint32_t n_tiles = W / p.paged.block_tokens;
   if (p.hnd) {
@@ -472,7 +483,7 @@ __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kThreads)
     // ([bs][D] rows are contiguous), so the warp streams the block with 16-byte loads, folds the lanes
     // with one REDUX and owns s_absmax[h] — no index arithmetic per vector, no atomics.
     const uint32_t lane = threadIdx.x & 31u;
-    for (uint32_t h = threadIdx.x >> 5; h < p.n_heads; h += kThreads >> 5) {
+    for (uint32_t h = threadIdx.x >> 5; h < p.n_heads; h += kFp8Threads >> 5) {
       uint32_t acc = 0;
       for (uint32_t tile = 0; tile < n_tiles; ++tile) {
         const uint32_t t0 = tile * p.paged.block_tokens;
@@ -490,10 +501,10 @@ __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kThreads)
   } else {
   // ---- per-head absmax over this CTA's tokens: a thread's 16-byte column has a fixed head ----
     // When a token has fewer than 256 vectors the spare threads split the tokens between them.
-    const uint32_t groups = vpt < kThreads ? kThreads / vpt : 1;
+    const uint32_t groups = vpt < kFp8Threads ? kFp8Threads / vpt : 1;
     const uint32_t grp = threadIdx.x / vpt;
     if (grp < groups) {
-      const uint32_t col_step = groups == 1 ? kThreads : vpt;
+      const uint32_t col_step = groups == 1 ? kFp8Threads : vpt;
       for (uint32_t col = threadIdx.x - grp * vpt; col < vpt; col += col_step) {
         uint32_t acc = 0;
         const uint8_t* q = smem + static_cast<size_t>(col) * 16;
@@ -502,7 +513,7 @@ __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kThreads)
           acc = absmax_u16x2(absmax_u16x2(absmax_u16x2(absmax_u16x2(acc, v.x), v.y), v.z), v.w);
         }
         const uint32_t m = max(acc & 0xffffu, acc >> 16);
-        atomicMax(&s_absmax[(col * 16) / p.head_bytes], m);
+        atomicMax(&s_absmax[(col * 16) / p.row_bytes], m);
       }
     }
   }
@@ -524,7 +535,7 @@ __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kThreads)
     const float inv = (m == 0) ? 1.0f : __fdiv_rn(448.0f, amax);
     s_inv[threadIdx.x] = inv;
     if (rank == 0) {
-      float* scales = reinterpret_cast<float*>(p.chunk_addrs[c] + p.scales_off);
+      float* scales = reinterpret_cast<float*>(p.chunk.chunk_addrs[c] + p.chunk.scales_off);
       scales[plane * p.n_heads + threadIdx.x] = (m == 0) ? 1.0f : __fdiv_rn(amax, 448.0f);
     }
   }
@@ -532,10 +543,10 @@ __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kThreads)
 
   if (p.hnd) {
     // the packed slab mirrors the tiles at half size: same vector index, 8 bytes each
-    uint8_t* outh = reinterpret_cast<uint8_t*>(p.chunk_addrs[c] + static_cast<uint64_t>(plane) * p.slab_q_bytes +
+    uint8_t* outh = reinterpret_cast<uint8_t*>(p.chunk.chunk_addrs[c] + static_cast<uint64_t>(plane) * p.chunk.slab_bytes +
                                                static_cast<uint64_t>(rank * W) * (tb >> 1));
     const uint32_t lane = threadIdx.x & 31u;
-    for (uint32_t h = threadIdx.x >> 5; h < p.n_heads; h += kThreads >> 5) {
+    for (uint32_t h = threadIdx.x >> 5; h < p.n_heads; h += kFp8Threads >> 5) {
       const float inv = s_inv[h];
       for (uint32_t tile = 0; tile < n_tiles; ++tile) {
         const uint32_t t0 = tile * p.paged.block_tokens;
@@ -552,21 +563,21 @@ __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kThreads)
   }
 
   // ---- quantise from smem, 8-byte coalesced stores ----
-  uint8_t* out = reinterpret_cast<uint8_t*>(p.chunk_addrs[c] + static_cast<uint64_t>(plane) * p.slab_q_bytes +
+  uint8_t* out = reinterpret_cast<uint8_t*>(p.chunk.chunk_addrs[c] + static_cast<uint64_t>(plane) * p.chunk.slab_bytes +
                                             static_cast<uint64_t>(rank * W) * (tb >> 1));
   const uint32_t nvec = n_valid * vpt;
-  if ((kThreads % vpt) == 0) {
+  if ((kFp8Threads % vpt) == 0) {
     // i % vpt == threadIdx.x % vpt for every i of this thread: one head, one scale, no division
-    const float inv = s_inv[((threadIdx.x % vpt) * 16) / p.head_bytes];
-    for (uint32_t i = threadIdx.x; i < nvec; i += kThreads) {
+    const float inv = s_inv[((threadIdx.x % vpt) * 16) / p.row_bytes];
+    for (uint32_t i = threadIdx.x; i < nvec; i += kFp8Threads) {
       const uint4 v = *reinterpret_cast<const uint4*>(smem + static_cast<size_t>(i) * 16);
       st_na_v2(out + static_cast<size_t>(i) * 8, quant8(v, inv));
     }
   } else {
-    for (uint32_t i = threadIdx.x; i < nvec; i += kThreads) {
+    for (uint32_t i = threadIdx.x; i < nvec; i += kFp8Threads) {
       const uint32_t col = i % vpt;
       const uint4 v = *reinterpret_cast<const uint4*>(smem + static_cast<size_t>(i) * 16);
-      st_na_v2(out + static_cast<size_t>(i) * 8, quant8(v, s_inv[(col * 16) / p.head_bytes]));
+      st_na_v2(out + static_cast<size_t>(i) * 8, quant8(v, s_inv[(col * 16) / p.row_bytes]));
     }
   }
 }
@@ -590,8 +601,10 @@ __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kThreads)
 // A group releases its buffer as soon as the unit is in registers, so while it reduces and quantises unit i its
 // unit i+2 is already streaming in, and so is the other group's: the memory pipe never drains between the load -> absmax -> quantise phases of a unit (the cluster kernel above
 // runs at 33 % warps active with exactly that bubble).  HBM is read once and written once.
-// Eligibility (checked on the host, else the cluster kernel runs): every chunk is a sequence of whole,
-// block-aligned runs, the last one possibly short — what any vLLM block table produces.
+// Eligibility (checked on the host, else the cluster kernel runs): the geometry fits the unit buffers, and every
+// chunk is a sequence of whole, block-aligned runs, the last one possibly short (whole_block_chunks in
+// b200kv_runs.h) — what any vLLM block table produces.  Run j of chunk c is then paged block j of the chunk.
+// total_units = n_chunks * n_planes * H.
 // ---------------------------------------------------------------------------------------------
 constexpr int kS3Groups = 2;
 constexpr int kS3Stages = kS3Groups;   // stage g is filled for, and drained by, consumer group g only: consecutive uses of a
@@ -602,20 +615,6 @@ constexpr int kS3GroupThreads = 256;
 constexpr int kS3Threads = 32 + kS3Groups * kS3GroupThreads;
 constexpr int kS3MaxVec = 16;          // 16-byte vectors per consumer thread per unit
 constexpr uint32_t kS3MaxUnitBytes = kS3MaxVec * kS3GroupThreads * 16;   // 64 KiB
-
-struct Fp8Store3Params {
-  PagedSide paged;
-  const Run* runs;                // run j of chunk c = paged block j of the chunk (host-checked)
-  const uint32_t* chunk_run_off;  // [n_chunks+1]
-  const uint64_t* chunk_addrs;    // [n_chunks]
-  const void* tmaps;              // device array of CUtensorMap, one per plane (NHD); nullptr: plain bulk copies (HND)
-  uint32_t n_chunks, n_planes;
-  uint32_t chunk_tokens, n_tokens;
-  uint32_t n_heads, head_bytes;   // H, D*2
-  uint64_t slab_q_bytes, scales_off;
-  uint32_t hnd;
-  uint32_t total_units;           // n_chunks * n_planes * H
-};
 
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
@@ -633,15 +632,16 @@ __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t n_threads) 
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n_threads) : "memory");
 }
 
-__global__ void __launch_bounds__(kS3Threads, 1) kv_fp8_store3_kernel(const Fp8Store3Params p) {
+__global__ void __launch_bounds__(kS3Threads, 1) kv_fp8_store3_kernel(const KernelArgs p,
+                     const void* tmaps) {   // one CUtensorMap per plane (NHD pages); nullptr for HND pages
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ __align__(8) uint64_t full_bar[kS3Stages];
   __shared__ __align__(8) uint64_t empty_bar[kS3Stages];
   __shared__ uint32_t s_max[kS3Groups][2][kS3GroupThreads / 32];
 
   const uint32_t bs = p.paged.block_tokens;
-  const uint32_t piece_bytes = bs * p.head_bytes;            // one block's rows of one head
-  const uint32_t unit_bytes = p.chunk_tokens * p.head_bytes;  // stage size (<= 64 KiB, host-checked)
+  const uint32_t piece_bytes = bs * p.row_bytes;                   // one block's rows of one head
+  const uint32_t unit_bytes = p.chunk.chunk_tokens * p.row_bytes;  // stage size (<= 64 KiB, host-checked)
   const uint32_t H = p.n_heads;
 
   if (threadIdx.x == 0) {
@@ -673,10 +673,9 @@ __global__ void __launch_bounds__(kS3Threads, 1) kv_fp8_store3_kernel(const Fp8S
       for (uint32_t j = lane; j < n_blocks; j += 32) {
         const uint32_t block = static_cast<uint32_t>(p.runs[r0 + j].a) / bs;
         uint8_t* dst = stage + static_cast<size_t>(j) * piece_bytes;
-        if (p.tmaps) {
-          const uint8_t* tm = static_cast<const uint8_t*>(p.tmaps) + static_cast<size_t>(plane) * 128;
-          if (p.hnd) tma_load_4d(dst, tm, 0, 0, static_cast<int32_t>(h), static_cast<int32_t>(block), &full_bar[s]);
-          else tma_load_4d(dst, tm, 0, static_cast<int32_t>(h), 0, static_cast<int32_t>(block), &full_bar[s]);
+        if (tmaps) {   // NHD pages
+          const uint8_t* tm = static_cast<const uint8_t*>(tmaps) + static_cast<size_t>(plane) * 128;
+          tma_load_4d(dst, tm, 0, static_cast<int32_t>(h), 0, static_cast<int32_t>(block), &full_bar[s]);
         } else {
           const uint64_t src = __ldg(p.paged.bases + plane) + static_cast<uint64_t>(block) * p.paged.block_stride +
                                static_cast<uint64_t>(h) * piece_bytes;   // HND tile [H][bs][D]
@@ -691,11 +690,11 @@ __global__ void __launch_bounds__(kS3Threads, 1) kv_fp8_store3_kernel(const Fp8S
   const uint32_t g = (threadIdx.x - 32) / kS3GroupThreads;
   const uint32_t t = (threadIdx.x - 32) % kS3GroupThreads;
   const uint32_t warp = t >> 5, lane = t & 31u;
-  const uint32_t rv = p.head_bytes >> 4;          // 16-byte vectors per (token, head) row; power of two (host-checked)
+  const uint32_t rv = p.row_bytes >> 4;          // 16-byte vectors per (token, head) row; power of two (host-checked)
   const uint32_t col8 = (t % rv) * 8;             // byte offset of this thread's 8 output bytes inside a row
   const uint32_t tok0 = t / rv;                   // token of vector kk = tok0 + kk * tok_step
   const uint32_t tok_step = kS3GroupThreads / rv;
-  const uint32_t out_row = p.head_bytes >> 1;     // D bytes of e4m3 per (token, head)
+  const uint32_t out_row = p.row_bytes >> 1;     // D bytes of e4m3 per (token, head)
   uint32_t it = 0;
   for (uint32_t i = g; i < n_mine; i += kS3Groups, ++it) {
     const uint32_t u = blockIdx.x + i * gridDim.x;
@@ -733,12 +732,12 @@ __global__ void __launch_bounds__(kS3Threads, 1) kv_fp8_store3_kernel(const Fp8S
     for (int w = 0; w < kS3GroupThreads / 32; ++w) m = max(m, s_max[g][par][w]);
     const float amax = __uint_as_float(m << 16);
     const float inv = (m == 0) ? 1.0f : __fdiv_rn(448.0f, amax);
-    const uint64_t chunk_base = __ldg(p.chunk_addrs + c);
+    const uint64_t chunk_base = __ldg(p.chunk.chunk_addrs + c);
     if (t == 0) {
-      float* scales = reinterpret_cast<float*>(chunk_base + p.scales_off);
+      float* scales = reinterpret_cast<float*>(chunk_base + p.chunk.scales_off);
       scales[plane * H + h] = (m == 0) ? 1.0f : __fdiv_rn(amax, 448.0f);
     }
-    uint8_t* slab = reinterpret_cast<uint8_t*>(chunk_base + static_cast<uint64_t>(plane) * p.slab_q_bytes);
+    uint8_t* slab = reinterpret_cast<uint8_t*>(chunk_base + static_cast<uint64_t>(plane) * p.chunk.slab_bytes);
     // output offset of vector kk is linear in kk: NHD [token][H][D]; HND [tile][H][bs][D] when a step of
     // tok_step tokens is a whole number of tiles (the host checks tok_step % bs == 0 before choosing this kernel)
     uint32_t off0, off_step;
@@ -759,22 +758,9 @@ __global__ void __launch_bounds__(kS3Threads, 1) kv_fp8_store3_kernel(const Fp8S
 }
 
 // ---------------------------------------------------------------------------------------------
-// FP8 load: one CTA per (run, plane) unit; e4m3 * scale -> bf16 (RN) into the pages.
+// FP8 load: one CTA per (run, plane) unit (total_units = n_runs * n_planes); e4m3 * scale -> bf16 (RN)
+// into the pages.
 // ---------------------------------------------------------------------------------------------
-struct Fp8LoadParams {
-  PagedSide paged;
-  const Run* runs;
-  const uint64_t* chunk_addrs;
-  uint32_t n_runs, n_planes;
-  uint32_t chunk_tokens;
-  uint32_t n_heads, head_bytes;  // head_bytes = D*2 (bf16 side)
-  uint64_t slab_q_bytes;
-  uint64_t scales_off;
-  uint32_t total_units;
-  uint32_t hnd;
-  uint32_t plane_begin;
-};
-
 __device__ __forceinline__ uint4 dequant8(const uint2& q, float scale) {
   const uint32_t w[2] = {q.x, q.y};
   uint32_t o[4];
@@ -792,7 +778,7 @@ __device__ __forceinline__ uint4 dequant8(const uint2& q, float scale) {
   return make_uint4(o[0], o[1], o[2], o[3]);
 }
 
-__global__ void __launch_bounds__(kFp8Threads) kv_fp8_load_kernel(const Fp8LoadParams p) {
+__global__ void __launch_bounds__(kFp8Threads) kv_fp8_load_kernel(const KernelArgs p) {
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ __align__(8) uint64_t bar;
   __shared__ float s_scale[kMaxHeads];
@@ -809,38 +795,38 @@ __global__ void __launch_bounds__(kFp8Threads) kv_fp8_load_kernel(const Fp8LoadP
   for (uint32_t ui = blockIdx.x; ui < p.total_units; ui += gridDim.x, phase ^= 1u) {
     const uint32_t plane = p.plane_begin + ui % p.n_planes;
     const Run run = p.runs[ui / p.n_planes];
-    const uint32_t c = static_cast<uint32_t>(run.b) / p.chunk_tokens;
-    const uint32_t t = static_cast<uint32_t>(run.b) - c * p.chunk_tokens;
-    const uint64_t cbase = __ldg(p.chunk_addrs + c);
+    const ChunkPos cp = chunk_pos(p.chunk, static_cast<uint32_t>(run.b));
+    const uint32_t t = cp.t;
+    const uint64_t cbase = __ldg(p.chunk.chunk_addrs + cp.c);
     const uint32_t bs = p.paged.block_tokens;
     // NHD: the run's n tokens are contiguous in the packed slab.  HND: fetch the whole packed tile
     // ([H][bs][D] bytes) the run lives in and pick its rows.
     const uint32_t q_off = p.hnd ? (t / bs) * bs * qtb : t * qtb;
     const uint32_t qbytes = p.hnd ? bs * qtb : static_cast<uint32_t>(run.n) * qtb;
     if (threadIdx.x == 0) {
-      bulk_g2s(smem, reinterpret_cast<const void*>(cbase + static_cast<uint64_t>(plane) * p.slab_q_bytes + q_off),
+      bulk_g2s(smem, reinterpret_cast<const void*>(cbase + static_cast<uint64_t>(plane) * p.chunk.slab_bytes + q_off),
                qbytes, &bar);
       mbar_arrive_expect_tx(&bar, qbytes);
     }
     if (threadIdx.x < p.n_heads)
       s_scale[threadIdx.x] =
-          reinterpret_cast<const float*>(cbase + p.scales_off)[plane * p.n_heads + threadIdx.x];
+          reinterpret_cast<const float*>(cbase + p.chunk.scales_off)[plane * p.n_heads + threadIdx.x];
     __syncthreads();
     mbar_wait(&bar, phase);
     const uint32_t vpt = tb >> 4;
     if (p.hnd) {
-      const uint32_t rv = p.head_bytes >> 4;          // 16-byte output vectors per (token, head) row
-      const uint32_t o_src = t % bs;                    // first row inside the packed tile
+      const uint32_t rv = p.row_bytes >> 4;   // 16-byte output vectors per (token, head) row
+      const uint32_t o_src = t % bs;          // first row inside the packed tile
       const uint32_t n = static_cast<uint32_t>(run.n);
       const uint32_t total = p.n_heads * n * rv;
       for (uint32_t e = threadIdx.x; e < total; e += kFp8Threads) {
         const uint32_t cc = e % rv;
         const uint32_t r = (e / rv) % n;
         const uint32_t h = e / (rv * n);
-        const uint2 q = *reinterpret_cast<const uint2*>(smem + (static_cast<size_t>(h) * bs + o_src + r) * (p.head_bytes >> 1) +
+        const uint2 q = *reinterpret_cast<const uint2*>(smem + (static_cast<size_t>(h) * bs + o_src + r) * (p.row_bytes >> 1) +
                                                         static_cast<size_t>(cc) * 8);
-        uint8_t* d = reinterpret_cast<uint8_t*>(paged_addr_hnd(p.paged, plane, static_cast<uint32_t>(run.a), h, p.head_bytes));
-        st_na_v4(d + static_cast<size_t>(r) * p.head_bytes + static_cast<size_t>(cc) * 16, dequant8(q, s_scale[h]));
+        uint8_t* d = reinterpret_cast<uint8_t*>(paged_addr_hnd(p.paged, plane, static_cast<uint32_t>(run.a), h, p.row_bytes));
+        st_na_v4(d + static_cast<size_t>(r) * p.row_bytes + static_cast<size_t>(cc) * 16, dequant8(q, s_scale[h]));
       }
       __syncthreads();
       continue;
@@ -848,7 +834,7 @@ __global__ void __launch_bounds__(kFp8Threads) kv_fp8_load_kernel(const Fp8LoadP
     uint8_t* dst = reinterpret_cast<uint8_t*>(paged_addr(p.paged, plane, static_cast<uint32_t>(run.a)));
     const uint32_t nvec = static_cast<uint32_t>(run.n) * vpt;
     if ((kFp8Threads % vpt) == 0) {
-      const float sc = s_scale[((threadIdx.x % vpt) * 16) / p.head_bytes];
+      const float sc = s_scale[((threadIdx.x % vpt) * 16) / p.row_bytes];
       for (uint32_t i = threadIdx.x; i < nvec; i += kFp8Threads) {
         const uint2 q = *reinterpret_cast<const uint2*>(smem + static_cast<size_t>(i) * 8);
         st_na_v4(dst + static_cast<size_t>(i) * 16, dequant8(q, sc));
@@ -857,7 +843,7 @@ __global__ void __launch_bounds__(kFp8Threads) kv_fp8_load_kernel(const Fp8LoadP
       for (uint32_t i = threadIdx.x; i < nvec; i += kFp8Threads) {
         const uint32_t col = i % vpt;
         const uint2 q = *reinterpret_cast<const uint2*>(smem + static_cast<size_t>(i) * 8);
-        st_na_v4(dst + static_cast<size_t>(i) * 16, dequant8(q, s_scale[(col * 16) / p.head_bytes]));
+        st_na_v4(dst + static_cast<size_t>(i) * 16, dequant8(q, s_scale[(col * 16) / p.row_bytes]));
       }
     }
     __syncthreads();  // smem + s_scale reusable
@@ -868,28 +854,17 @@ __global__ void __launch_bounds__(kFp8Threads) kv_fp8_load_kernel(const Fp8LoadP
 // Q4: group-wise 4-bit format (B200KV_FMT_Q4; oracle: q4_pack_chunk / q4_unpack_chunk).  A stored
 // token of one plane is a record [H*D/2 code bytes][H*D/32 bf16 scales]; records are token-major in the
 // slab whatever the order inside the paged tiles.  One 16-byte vector (8 elements) per thread, a group
-// of 32 elements = 4 adjacent lanes: absmax by two shuffles, no shared memory, no cluster.
-// EXPERIMENTAL: written against the oracle, not yet run on a GPU.
+// of 32 elements = 4 adjacent lanes: absmax by two shuffles, no shared memory, no cluster.  One unit per
+// (run, plane): total_units = n_runs * n_planes.  chunk.token_bytes is the record size, H*D/2 + H*D/32*2.
+// Bit-exact against the oracle on an H100 (tests/test_gpu_q4.py); still instruction-bound, the address
+// arithmetic is done per vector (DESIGN §3, §5).
 // ---------------------------------------------------------------------------------------------
-struct Q4Params {
-  PagedSide paged;
-  const Run* runs;
-  const uint64_t* chunk_addrs;
-  uint32_t n_runs, n_planes, plane_begin;
-  uint32_t chunk_tokens;
-  uint32_t n_heads, head_bytes;   // head_bytes = D*2 (bf16 side)
-  uint64_t slab_bytes;            // C * rec_bytes
-  uint32_t rec_bytes;             // H*D/2 + H*D/32*2
-  uint32_t total_units;           // n_runs * n_planes
-  uint32_t hnd;
-};
-
-__device__ __forceinline__ uint64_t q4_src_addr(const Q4Params& p, uint32_t plane, uint32_t slot, uint32_t v) {
+__device__ __forceinline__ uint64_t q4_src_addr(const KernelArgs& p, uint32_t plane, uint32_t slot, uint32_t v) {
   // v = 16-byte vector index inside the token: head h = v / rv, vector c of that head
   if (!p.hnd) return paged_addr(p.paged, plane, slot) + static_cast<uint64_t>(v) * 16;
-  const uint32_t rv = p.head_bytes >> 4;
+  const uint32_t rv = p.row_bytes >> 4;
   const uint32_t h = v / rv, c = v - h * rv;
-  return paged_addr_hnd(p.paged, plane, slot, h, p.head_bytes) + static_cast<uint64_t>(c) * 16;
+  return paged_addr_hnd(p.paged, plane, slot, h, p.row_bytes) + static_cast<uint64_t>(c) * 16;
 }
 
 constexpr int kQ4Unroll = 4;   // 16-byte vectors a thread keeps in flight (the kernels are pure streaming)
@@ -901,16 +876,17 @@ __device__ __forceinline__ void q4_split(uint32_t idx, uint32_t vpt, uint32_t vp
 
 // q = rint(x * inv) (exact product, ties to even), inv = fl32(1 / s), s = bf16(absmax_group / 7)
 // (oracle/kv_oracle.py q4_pack_chunk): one IEEE division per group, then one FMA per element.
-__global__ void __launch_bounds__(256) kv_q4_store_kernel(const Q4Params p) {
-  const uint32_t vpt = (p.n_heads * p.head_bytes) >> 4;      // vectors per token (multiple of 4)
+__global__ void __launch_bounds__(256) kv_q4_store_kernel(const KernelArgs p) {
+  const uint32_t vpt = (p.n_heads * p.row_bytes) >> 4;      // vectors per token (multiple of 4)
   const uint32_t vpt_shift = (vpt & (vpt - 1)) == 0 ? 31u - __clz(vpt) : 0xffffffffu;
   const uint32_t codes_bytes = vpt * 4;
   for (uint32_t ui = blockIdx.x; ui < p.total_units; ui += gridDim.x) {
     const uint32_t plane = p.plane_begin + ui % p.n_planes;
     const Run run = p.runs[ui / p.n_planes];
-    const uint32_t c = static_cast<uint32_t>(run.b) / p.chunk_tokens;
-    const uint32_t t0 = static_cast<uint32_t>(run.b) - c * p.chunk_tokens;
-    uint8_t* slab = reinterpret_cast<uint8_t*>(__ldg(p.chunk_addrs + c) + static_cast<uint64_t>(plane) * p.slab_bytes);
+    const ChunkPos cp = chunk_pos(p.chunk, static_cast<uint32_t>(run.b));
+    const uint32_t t0 = cp.t;
+    uint8_t* slab =
+        reinterpret_cast<uint8_t*>(__ldg(p.chunk.chunk_addrs + cp.c) + static_cast<uint64_t>(plane) * p.chunk.slab_bytes);
     const uint32_t nvec = static_cast<uint32_t>(run.n) * vpt;
     for (uint32_t base = 0; base < nvec; base += 256 * kQ4Unroll) {   // uniform trip count: every lane shuffles
       uint4 x[kQ4Unroll];
@@ -947,7 +923,7 @@ __global__ void __launch_bounds__(256) kv_q4_store_kernel(const Q4Params p) {
           packed |= (ql | (qh << 4)) << (8 * i);
         }
         if (!ok[j]) continue;
-        uint8_t* rec = slab + static_cast<uint64_t>(t0 + tt[j]) * p.rec_bytes;
+        uint8_t* rec = slab + static_cast<uint64_t>(t0 + tt[j]) * p.chunk.token_bytes;
         *reinterpret_cast<uint32_t*>(rec + static_cast<size_t>(vv[j]) * 4) = packed;
         if ((vv[j] & 3u) == 0) *reinterpret_cast<__nv_bfloat16*>(rec + codes_bytes + static_cast<size_t>(vv[j] >> 2) * 2) = sb;
       }
@@ -955,17 +931,17 @@ __global__ void __launch_bounds__(256) kv_q4_store_kernel(const Q4Params p) {
   }
 }
 
-__global__ void __launch_bounds__(256) kv_q4_load_kernel(const Q4Params p) {
-  const uint32_t vpt = (p.n_heads * p.head_bytes) >> 4;
+__global__ void __launch_bounds__(256) kv_q4_load_kernel(const KernelArgs p) {
+  const uint32_t vpt = (p.n_heads * p.row_bytes) >> 4;
   const uint32_t vpt_shift = (vpt & (vpt - 1)) == 0 ? 31u - __clz(vpt) : 0xffffffffu;
   const uint32_t codes_bytes = vpt * 4;
   for (uint32_t ui = blockIdx.x; ui < p.total_units; ui += gridDim.x) {
     const uint32_t plane = p.plane_begin + ui % p.n_planes;
     const Run run = p.runs[ui / p.n_planes];
-    const uint32_t c = static_cast<uint32_t>(run.b) / p.chunk_tokens;
-    const uint32_t t0 = static_cast<uint32_t>(run.b) - c * p.chunk_tokens;
-    const uint8_t* slab =
-        reinterpret_cast<const uint8_t*>(__ldg(p.chunk_addrs + c) + static_cast<uint64_t>(plane) * p.slab_bytes);
+    const ChunkPos cp = chunk_pos(p.chunk, static_cast<uint32_t>(run.b));
+    const uint32_t t0 = cp.t;
+    const uint8_t* slab = reinterpret_cast<const uint8_t*>(__ldg(p.chunk.chunk_addrs + cp.c) +
+                                                           static_cast<uint64_t>(plane) * p.chunk.slab_bytes);
     const uint32_t nvec = static_cast<uint32_t>(run.n) * vpt;
     for (uint32_t base = threadIdx.x; base < nvec; base += 256 * kQ4Unroll) {
       uint32_t packed[kQ4Unroll], tt[kQ4Unroll], vv[kQ4Unroll];
@@ -978,7 +954,7 @@ __global__ void __launch_bounds__(256) kv_q4_load_kernel(const Q4Params p) {
         tt[j] = vv[j] = 0;
         if (idx < nvec) {
           q4_split(idx, vpt, vpt_shift, &tt[j], &vv[j]);
-          const uint8_t* rec = slab + static_cast<uint64_t>(t0 + tt[j]) * p.rec_bytes;
+          const uint8_t* rec = slab + static_cast<uint64_t>(t0 + tt[j]) * p.chunk.token_bytes;
           packed[j] = __ldg(reinterpret_cast<const uint32_t*>(rec + static_cast<size_t>(vv[j]) * 4));
           sbits[j] = __ldg(reinterpret_cast<const uint16_t*>(rec + codes_bytes + static_cast<size_t>(vv[j] >> 2) * 2));
         }

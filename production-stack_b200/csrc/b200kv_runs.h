@@ -142,6 +142,28 @@ inline int build_op_table(const int64_t* slots, const Span* spans, size_t n_span
   return B200KV_OK;
 }
 
+// True if every chunk of `t` is a sequence of whole, block-aligned runs, only the last one possibly short: run j
+// of chunk c starts at op-relative token c*C + j*bs and at the first slot of a block.  Any vLLM block table gives
+// such a table; the persistent FP8 store (kv_fp8_store3_kernel) takes no other.  Reads the full runs only.
+inline bool whole_block_chunks(const OpTable& t, int32_t bs, int32_t C) {
+  const uint32_t ubs = static_cast<uint32_t>(bs), uc = static_cast<uint32_t>(C);
+  for (uint32_t c = 0; c < t.n_chunks(); ++c) {
+    const uint32_t r0 = t.full_off[c], r1 = t.full_off[c + 1];
+    uint32_t n_valid = 0;   // the chunk's tokens: its runs cover them
+    for (uint32_t r = r0; r < r1; ++r) n_valid += static_cast<uint32_t>(t.runs[r].n);
+    if (n_valid == 0 || n_valid > uc) return false;
+    const uint32_t nb = (n_valid + ubs - 1) / ubs;
+    if (r1 - r0 != nb) return false;
+    for (uint32_t j = 0; j < nb; ++j) {
+      const Run& run = t.runs[r0 + j];
+      if (run.b != static_cast<int32_t>(c * uc + j * ubs) || static_cast<uint32_t>(run.a) % ubs != 0 ||
+          static_cast<uint32_t>(run.n) != std::min(ubs, n_valid - j * ubs))
+        return false;
+    }
+  }
+  return true;
+}
+
 // Byte layout of a table as the kernels read it: the runs, the chunk addresses, then full_off (the FP8
 // store kernels' per-chunk run offsets), each rounded up to 16 bytes.  A table over kTableBytes is refused.
 constexpr size_t kTableBytes = 1u << 20;

@@ -59,6 +59,13 @@ extern "C" int table_layout(int64_t n_runs, int64_t n_chunks, uint64_t* l) {
   return rc;
 }
 
+extern "C" int whole_block(const Run* runs, const uint32_t* full_off, int64_t n_chunks, int32_t bs, int32_t C) {
+  b200kv::OpTable t;
+  t.full_off.assign(full_off, full_off + n_chunks + 1);
+  t.runs.assign(runs, runs + full_off[n_chunks]);
+  return b200kv::whole_block_chunks(t, bs, C);
+}
+
 extern "C" int pull_runs(const int64_t* src, const int64_t* dst, int64_t n, int64_t max_src, int64_t max_dst,
                          int32_t bs, int hnd, Run* full, int64_t* n_full, Run* part, int64_t* n_part) {
   std::vector<Run> f, p;
@@ -393,3 +400,102 @@ def test_table_layout_and_its_cap(lib):
             assert layout(n_runs, n_chunks) == ((0 if total <= 1 << 20 else EINVAL), [0, runs, runs + addrs, total])
     assert layout(87378, 1) == (0, [0, 1048544, 1048560, 1 << 20])      # one chunk: exactly 1 MiB
     assert layout(87379, 1)[0] == EINVAL
+
+
+def whole_block(lib, runs, full_off, bs, c):
+    runs = np.ascontiguousarray(np.asarray(runs, np.int32).reshape(-1, 3))
+    off = np.ascontiguousarray(full_off, np.uint32)
+    return bool(lib.whole_block(_p(runs), _p(off), C.c_int64(len(off) - 1), C.c_int32(bs), C.c_int32(c)))
+
+
+def ref_whole_block(runs, full_off, bs, c):
+    """Chunk k's runs are its paged blocks in order: run j starts at op-relative token k*C + j*bs and at a block's
+    first slot, and holds bs tokens, or the chunk's remaining tokens if it is the last run."""
+    for k in range(len(full_off) - 1):
+        rs = runs[full_off[k]:full_off[k + 1]]
+        n = sum(r[2] for r in rs)
+        if n == 0 or n > c or len(rs) != -(-n // bs):
+            return False
+        for j, (a, b, m) in enumerate(rs):
+            if b != k * c + j * bs or a % bs or m != min(bs, n - j * bs):
+                return False
+    return True
+
+
+def fp8_table(lib, slots, spans, nb, bs, c, hnd):
+    """The table an FP8 op builds (no partial-tile split)."""
+    rc, runs, full_off, _ = build_table(lib, slots, spans, nb * bs, bs, c, False, hnd)
+    assert rc == 0
+    return runs, full_off
+
+
+@pytest.mark.parametrize("hnd", [False, True])
+@pytest.mark.parametrize("bs,c", [(16, 256), (16, 64), (8, 32), (16, 16)])
+def test_whole_block_chunks_accepts_block_tables(lib, bs, c, hnd):
+    """Batches of requests over block tables: every request's last chunk is short and may end mid-block, and
+    the next request's chunks follow it in the same table."""
+    nb = 512
+    rng = np.random.default_rng(40 + bs + c + hnd)
+    perm = rng.permutation(nb)
+    sm, spans, used = [], [], 0
+    for n_req in (c + 5, 2 * c, 3 * c + 1, bs + 3, c, 1, 2 * c - 1):
+        nblk = (n_req + bs - 1) // bs
+        req = block_map(perm[used:used + nblk], n_req, bs)
+        used += nblk
+        for k in range(0, n_req, c):
+            t = req[k:k + c]
+            spans.append((len(sm) * c, len(t)))
+            sm.append(np.concatenate([t, np.zeros(c - len(t), np.int64)]))
+    sm = np.concatenate(sm)
+    runs, full_off = fp8_table(lib, sm, spans, nb, bs, c, hnd)
+    assert any(n % bs for _, n in spans) and any(n < c for _, n in spans[:-1])
+    assert ref_whole_block(runs, full_off, bs, c)
+    assert whole_block(lib, runs, full_off, bs, c)
+    # gather-shaped: one request, chunks [k*C, (k+1)*C) of the op
+    n = 5 * c + bs // 2
+    slots = block_map(rng.permutation(nb)[:(n + bs - 1) // bs], n, bs)
+    runs, full_off = fp8_table(lib, slots, [(k, min(c, n - k)) for k in range(0, n, c)], nb, bs, c, hnd)
+    assert whole_block(lib, runs, full_off, bs, c)
+
+
+@pytest.mark.parametrize("hnd", [False, True])
+def test_whole_block_chunks_refuses_other_tables(lib, hnd):
+    bs, c, nb = 16, 64, 256
+    rng = np.random.default_rng(77 + hnd)
+    n = 3 * c
+    token_granular = rng.permutation(nb * bs)[:n]
+    mid_block = block_map(rng.permutation(nb)[:20], n, bs, start=5)        # a request entered mid-block
+    for slots in (token_granular, mid_block):
+        runs, full_off = fp8_table(lib, slots, [(k, c) for k in range(0, n, c)], nb, bs, c, hnd)
+        assert not ref_whole_block(runs, full_off, bs, c)
+        assert not whole_block(lib, runs, full_off, bs, c)
+    good = [(0, 0, 16), (32, 16, 16), (64, 32, 5)]                           # one chunk of 37 tokens
+    assert whole_block(lib, good, [0, 3], bs, c)
+    for bad in ([(0, 0, 16), (32, 16, 8), (64, 24, 13)],                     # a short run that is not the last
+                [(0, 0, 16), (32, 32, 16), (64, 48, 5)],                     # run 1 skips block position 1
+                [(0, 0, 16), (36, 16, 16), (64, 32, 5)],                     # run 1 starts mid-block
+                [(0, 0, 16), (32, 16, 16), (64, 32, 5), (80, 37, 1)]):       # more runs than blocks
+        assert not ref_whole_block(bad, [0, len(bad)], bs, c)
+        assert not whole_block(lib, bad, [0, len(bad)], bs, c)
+    assert not whole_block(lib, good + [(96, 64, 16)], [0, 3, 3], bs, c)     # an empty chunk
+    assert whole_block(lib, good + [(96, 64, 16)], [0, 3, 4], bs, c)         # chunk 1 at token C
+
+
+@pytest.mark.parametrize("hnd", [False, True])
+def test_whole_block_chunks_matches_its_restatement(lib, hnd):
+    bs, c, nb = 16, 64, 64
+    rng = np.random.default_rng(300 + hnd)
+    seen = set()
+    for _ in range(300):
+        n_op = int(rng.integers(1, 6))
+        if rng.integers(0, 2):
+            slots = random_map(rng, n_op * c, nb, bs)
+        else:
+            start = int(rng.integers(0, bs)) if rng.integers(0, 2) else 0
+            slots = block_map(rng.permutation(nb), n_op * c, bs, start=start)
+        spans = [(k * c, int(rng.integers(1, c + 1))) for k in range(n_op)]
+        runs, full_off = fp8_table(lib, slots, spans, nb, bs, c, hnd)
+        want = ref_whole_block(runs, full_off, bs, c)
+        seen.add(want)
+        assert whole_block(lib, runs, full_off, bs, c) == want
+    assert seen == {False, True}
