@@ -71,6 +71,19 @@ extern "C" {
  *      of the pool's per-chunk format tag).                                                  */
 #define B200KV_LAYOUT_NHD 0
 #define B200KV_LAYOUT_HND 1
+/* MLA: multi-head latent attention (DeepSeek-V2/V3, Kimi-K2).  ONE plane per layer, not a K and a V
+ *      plane: vLLM's MLA backends allocate (num_blocks, block_size, head_size) per layer
+ *      (MLACommonBackend.get_kv_cache_shape), so the tile is [block_tokens][D] and n_kv_heads must be 1.
+ *      A RAW chunk is (L, 1, C, 1, D) — LMCache's MLA kv_shape (vllm_v1_adapter.py:463-477).
+ *      FP8 on an MLA engine is a per-token latent record instead of the per-head format above: 656 bytes
+ *      per (token, layer), the byte layout of vLLM's fp8_ds_mla cache entry
+ *      (v1/attention/backends/mla/flashmla_sparse.py:68-79):
+ *        [0, 512)    e4m3 codes of latent elements 0..511
+ *        [512, 528)  4 fp32 scales, scale g = absmax(elements [128g, 128g+128)) / 448 (1 if absmax is 0)
+ *        [528, 656)  RoPE elements 512..575, bf16 bits copied verbatim
+ *      A chunk is L slabs of C records (no separate scales area), rounded up to 256 bytes.  Needs a bf16
+ *      cache and D == 576; Q4 is not offered on MLA (-ENOTSUP).                                  */
+#define B200KV_LAYOUT_MLA 2
 
 /* ---- kernel variants (both are CUDA; selectable for A/B measurement) ------------------- */
 #define B200KV_VARIANT_BULK 0 /* cp.async.bulk (TMA engine) through a shared-memory ring    */
@@ -233,7 +246,8 @@ int64_t b200kv_engine_chunk_bytes(const b200kv_engine_config* cfg);
 /* register_kv_caches (KVConnectorBase_V1, vllm/.../v1/base.py:251): device base address of
  * block 0 of each layer's K and V planes, NHD within a block ([block_tokens][H][D]).
  * FlashAttention (2,NB,bs,H,D): v = k + NB*tile; FlashInfer (NB,2,bs,H,D): v = k + tile,
- * block_stride = 2*tile; cross-layer (NB,L,2,bs,H,D): block_stride = 2*L*tile.             */
+ * block_stride = 2*tile; cross-layer (NB,L,2,bs,H,D): block_stride = 2*L*tile.
+ * B200KV_LAYOUT_MLA: k_ptrs are the layers' latent planes and v_ptrs must be NULL.           */
 int b200kv_register_kv(b200kv_ctx* ctx, const void* const* k_ptrs, const void* const* v_ptrs);
 
 /* lmcache_engine.store (vllm_v1_adapter.py:1115-1123).  Tokens [0,n_tokens) start on a
@@ -310,7 +324,9 @@ typedef struct b200kv_ipc_desc {
   uint64_t alloc_bytes; /* size of the allocation (informational)                            */
 } b200kv_ipc_desc;
 
-/* Export 2*L descriptors (K planes then V planes) of the registered cache.                 */
+/* Export 2*L descriptors (K planes then V planes) of the registered cache; L (one per layer's
+ * latent plane) for B200KV_LAYOUT_MLA.  import_peer takes as many; import_peer_ptrs takes
+ * v_ptrs NULL for MLA.                                                                     */
 int b200kv_export_ipc(b200kv_ctx* ctx, b200kv_ipc_desc* descs_out, int32_t n_descs);
 /* Map a peer replica's cache (same model geometry).  `peer_id` is caller-chosen (0..63).   */
 int b200kv_import_peer(b200kv_ctx* ctx, int32_t peer_id, int32_t peer_device,

@@ -14,7 +14,7 @@ LIB_PATH = os.path.join(_HERE, "libb200kv.so")
 
 FMT_RAW, FMT_FP8, FMT_Q4 = 0, 1, 2   # FMT_Q4: experimental (group-wise 4-bit)
 VARIANT_BULK, VARIANT_LDG = 0, 1
-LAYOUT_NHD, LAYOUT_HND = 0, 1
+LAYOUT_NHD, LAYOUT_HND, LAYOUT_MLA = 0, 1, 2   # LAYOUT_MLA: one latent plane per layer (DeepSeek-V2/V3, Kimi-K2)
 POOL_CREATE, POOL_ATTACH, POOL_CREATE_OR_ATTACH = 1, 2, 3
 NUMA_LOCAL, NUMA_INTERLEAVE, NUMA_OFF = 0, 1, 2
 

@@ -352,9 +352,13 @@ class WorkerStats:
 class WorkerState:
     """Worker-role half: turns ReqMeta into engine.store / engine.retrieve calls."""
 
-    def __init__(self, engine, block_size: int, chunk: int, kv_role: str = "kv_both", owner_tag: int = 0):
+    def __init__(self, engine, block_size: int, chunk: int, kv_role: str = "kv_both", owner_tag: int = 0,
+                 stores: bool = True):
         self.engine = engine
         self.owner_tag = owner_tag   # != 0: count tokens served from chunks stored under another owner tag
+        # False on tensor-parallel ranks > 0 of an MLA model: the latent is the same on every rank, so rank 0's
+        # copy in the host pool serves all of them and the other ranks only load
+        self.stores = stores
         self.block_size = block_size
         self.chunk = chunk
         self.kv_role = kv_role
@@ -540,7 +544,7 @@ class WorkerState:
     def save(self, metas: list[ReqMeta], stream=None):
         """wait_for_save (adapter :1033-1128).  Blocks only until the gather kernels are queued;
         the caller's stream is made to wait for them, the D2H runs behind."""
-        if self.kv_role == "kv_consumer":
+        if self.kv_role == "kv_consumer" or not self.stores:
             return
         work = []     # (meta, tokens, sm, lead, n)
         for m in metas:

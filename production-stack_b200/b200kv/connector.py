@@ -71,16 +71,20 @@ class B200KVConnectorMetadata(KVConnectorMetadata):
 
 def geometry_from_vllm(vllm_config, cfg: B200KVConfig, n_blocks: int = 1) -> KVGeometry:
     """LMCache's kv_shape = (num_layer, 2, chunk, num_kv_head, head_size)
-    (vllm_v1_adapter.py:471-477), derivable in both roles from the vLLM config alone."""
+    (vllm_v1_adapter.py:471-477), derivable in both roles from the vLLM config alone.  An MLA model
+    (model_config.use_mla) has one latent plane per layer: (num_layer, 1, chunk, 1, head_size)
+    (vllm_v1_adapter.py:463-477)."""
     mc, pc, cc = vllm_config.model_config, vllm_config.parallel_config, vllm_config.cache_config
     dt = str(cc.cache_dtype)
     if dt in ("auto", "None"):
         elem = torch.empty((), dtype=mc.dtype).element_size()
     else:
         elem = 1 if "fp8" in dt else 2
-    return KVGeometry(n_layers=mc.get_num_layers(pc), n_kv_heads=mc.get_num_kv_heads(pc),
+    mla = bool(getattr(mc, "use_mla", False))
+    return KVGeometry(n_layers=mc.get_num_layers(pc), n_kv_heads=1 if mla else mc.get_num_kv_heads(pc),
                       head_dim=mc.get_head_size(), n_blocks=n_blocks, block_tokens=cc.block_size,
-                      chunk_tokens=cfg.chunk_size, elem_bytes=elem, block_stride_bytes=0, fmt=cfg.fmt)
+                      chunk_tokens=cfg.chunk_size, elem_bytes=elem, block_stride_bytes=0, fmt=cfg.fmt,
+                      layout=_lib.LAYOUT_MLA if mla else _lib.LAYOUT_NHD)
 
 
 def owner_tag_of(instance_id: str) -> int:
@@ -190,7 +194,8 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
                                          self.cfg.save_decode_cache, self.kv_role, async_load=self.cfg.async_load,
                                          priority_limit=self.cfg.priority_limit)
             if self.kv_role != "kv_producer":     # the scheduler fetches every TP rank's chunks of a prompt
-                self._remote = self._make_remote([self._key_seed(r) for r in range(self._world)])
+                # (one seed for MLA: every rank loads the same latent chunks)
+                self._remote = self._make_remote(list(dict.fromkeys(self._key_seed(r) for r in range(self._world))))
             if not self.cfg.pool_name:
                 # a per-engine segment dies with its engine (vLLM's engine ids are random: nobody would
                 # ever attach to it again); a named, shared one stays for the other replicas of the box
@@ -253,7 +258,8 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
         self._layer_index = {name: i for i, name in enumerate(kv_caches.keys())}
         self._layer_hooks_seen = 0
         self._worker = WorkerState(self._engine, self._block_size, self._chunk, self.kv_role,
-                                   owner_tag=owner_tag_of(self.cfg.instance_id) if self.cfg.pool_name else 0)
+                                   owner_tag=owner_tag_of(self.cfg.instance_id) if self.cfg.pool_name else 0,
+                                   stores=not geom.mla or self._tp_rank() == 0)   # MLA: rank 0 stores for all ranks
         if self.cfg.device_tier_gb > 0:
             from .device_tier import LocalTier, TierSet
             fmt_tag = self.cfg.fmt | (tile_layout << 8)

@@ -24,6 +24,7 @@ from . import _lib
 from ._lib import FMT_FP8, FMT_RAW, VARIANT_BULK, check, lib
 
 DEFAULT_SEED = 0x6232303030304B56  # keys are namespaced further by KVGeometry.key_seed()
+MLA_FP8_RECORD_BYTES = 656         # one (token, layer) of an MLA FP8 chunk (include/b200kv.h, B200KV_LAYOUT_MLA)
 
 
 def _as_i64(a) -> np.ndarray:
@@ -71,11 +72,20 @@ class KVGeometry:
     elem_bytes: int = 2
     block_stride_bytes: int = 0   # 0 -> dense (block_tokens * H * D * elem)
     fmt: int = FMT_RAW
-    layout: int = 0               # LAYOUT_NHD / LAYOUT_HND inside a block
+    layout: int = 0               # LAYOUT_NHD / LAYOUT_HND inside a block, or LAYOUT_MLA
 
     @property
     def token_bytes(self) -> int:
         return self.n_kv_heads * self.head_dim * self.elem_bytes
+
+    @property
+    def mla(self) -> bool:
+        return self.layout == _lib.LAYOUT_MLA
+
+    @property
+    def planes(self) -> int:
+        """Paged planes the engine moves: a K and a V plane per layer, or one latent plane (MLA)."""
+        return self.n_layers * (1 if self.mla else 2)
 
     @property
     def stride(self) -> int:
@@ -83,7 +93,11 @@ class KVGeometry:
 
     def key_seed(self, model: str = "", world_size: int = 1, rank: int = 0) -> int:
         """Namespace for chunk keys: same role as LMCache's CacheEngineKey(fmt, model, world_size,
-        worker_id, ...) — chunks of different models / shards / formats never alias."""
+        worker_id, ...) — chunks of different models / shards / formats never alias.  An MLA latent is
+        the same on every tensor-parallel rank, so its namespace keeps only the pipeline stage
+        (rank // world_size) of the rank: one stored copy serves every rank of the stage."""
+        if self.mla:
+            rank //= max(world_size, 1)
         tag = f"{model}|{world_size}|{rank}|{self.n_layers}|{self.n_kv_heads}|{self.head_dim}|" \
               f"{self.elem_bytes}|{self.chunk_tokens}|{self.fmt}|{self.layout}".encode()
         return xxh64(tag, DEFAULT_SEED)
@@ -103,11 +117,11 @@ class KVGeometry:
     @property
     def payload_bytes_per_token(self) -> int:
         """Bytes one token occupies in a stored chunk (SURVEY.md §8d 'payload P')."""
-        per = 2 * self.n_layers * self.token_bytes
+        per = self.planes * self.token_bytes
         if self.fmt == FMT_RAW:
             return per
         if self.fmt == FMT_FP8:
-            return per // 2
+            return self.n_layers * MLA_FP8_RECORD_BYTES if self.mla else per // 2
         return per * 9 // 32          # Q4: 4 bits + one bf16 scale per 32 elements = 4.5 bits per element
 
 
@@ -252,10 +266,19 @@ def _stream_ptr(stream) -> C.c_void_p:
 def paged_layout_of(t, block_tokens: int, layout: str | None = None):
     """(k_ptr, v_ptr, block_stride_bytes, n_blocks, H, D, tile_layout) of one layer's paged KV tensor.
     FlashAttention (2, NB, bs, H, D) (vllm/v1/attention/backends/flash_attn.py:140-149) or
-    FlashInfer (NB, 2, bs, H, D) (flashinfer.py:357-368); within a block the order must be NHD."""
-    if t.dim() != 5:
-        raise NotImplementedError(f"unsupported KV cache rank {t.dim()} (MLA / packed layouts)")
+    FlashInfer (NB, 2, bs, H, D) (flashinfer.py:357-368); within a block the order must be NHD or HND.
+    MLA (NB, bs, D) (MLACommonBackend.get_kv_cache_shape, model_executor/layers/attention/mla_attention.py):
+    one latent plane, v_ptr None, H 1, LAYOUT_MLA."""
     es = t.element_size()
+    if t.dim() == 3:
+        nb, bs, d = t.shape
+        if bs != block_tokens:
+            raise ValueError(f"MLA KV cache shape {tuple(t.shape)} does not match block size {block_tokens}")
+        if tuple(t.stride()[1:]) != (d, 1) or t.stride(0) < bs * d:
+            raise NotImplementedError("unsupported order inside an MLA KV block (strides %s)" % (tuple(t.stride()),))
+        return t.data_ptr(), None, t.stride(0) * es, nb, 1, d, _lib.LAYOUT_MLA
+    if t.dim() != 5:
+        raise NotImplementedError(f"unsupported KV cache rank {t.dim()} (packed layouts)")
     if layout is None:
         layout = "fa" if (t.shape[0] == 2 and t.shape[2] == block_tokens) else "fi"
     if layout == "fa":
@@ -295,12 +318,20 @@ class KVEngine:
         self._kv_refs = None
 
     # ---- registration ---------------------------------------------------------------------
-    def register_kv_ptrs(self, k_ptrs, v_ptrs):
+    def _plane_ptrs(self, k_ptrs, v_ptrs):
+        """ctypes arrays of the K and V pointers; MLA takes one latent pointer per layer and v_ptrs None."""
         L = self.geom.n_layers
-        if len(k_ptrs) != L or len(v_ptrs) != L:
+        if self.geom.mla:
+            if len(k_ptrs) != L or v_ptrs is not None:
+                raise ValueError("MLA: need one latent pointer per layer and no V pointers")
+            return (C.c_void_p * L)(*[C.c_void_p(int(p)) for p in k_ptrs]), None
+        if len(k_ptrs) != L or v_ptrs is None or len(v_ptrs) != L:
             raise ValueError("need one K and one V pointer per layer")
-        ka = (C.c_void_p * L)(*[C.c_void_p(int(p)) for p in k_ptrs])
-        va = (C.c_void_p * L)(*[C.c_void_p(int(p)) for p in v_ptrs])
+        return ((C.c_void_p * L)(*[C.c_void_p(int(p)) for p in k_ptrs]),
+                (C.c_void_p * L)(*[C.c_void_p(int(p)) for p in v_ptrs]))
+
+    def register_kv_ptrs(self, k_ptrs, v_ptrs):
+        ka, va = self._plane_ptrs(k_ptrs, v_ptrs)
         check(lib().b200kv_register_kv(self._h, ka, va), "b200kv_register_kv")
 
     def register_kv_caches(self, kv_caches, layout: str | None = None):
@@ -316,7 +347,7 @@ class KVEngine:
             ks.append(k)
             vs.append(v)
         self._kv_refs = tensors  # keep the storage alive
-        self.register_kv_ptrs(ks, vs)
+        self.register_kv_ptrs(ks, None if self.geom.mla else vs)
 
     # ---- LMCache-shaped data path ---------------------------------------------------------
     def _keys(self, tokens) -> np.ndarray:
@@ -487,14 +518,14 @@ class KVEngine:
                                           _stream_ptr(stream)), "b200kv_scatter_chunks")
 
     def export_ipc(self) -> bytes:
-        n = 2 * self.geom.n_layers
+        n = self.geom.planes
         arr = (_lib.IpcDesc * n)()
         check(lib().b200kv_export_ipc(self._h, arr, n), "b200kv_export_ipc")
         return bytes(arr)
 
     def import_peer(self, peer_id: int, peer_device: int, descs: bytes,
                     peer_block_stride: int | None = None, peer_n_blocks: int | None = None):
-        n = 2 * self.geom.n_layers
+        n = self.geom.planes
         arr = (_lib.IpcDesc * n).from_buffer_copy(descs)
         check(lib().b200kv_import_peer(self._h, peer_id, peer_device, arr, n,
                                         peer_block_stride or self.geom.stride,
@@ -502,9 +533,7 @@ class KVEngine:
 
     def import_peer_ptrs(self, peer_id: int, peer_device: int, k_ptrs, v_ptrs,
                          peer_block_stride: int | None = None, peer_n_blocks: int | None = None):
-        L = self.geom.n_layers
-        ka = (C.c_void_p * L)(*[C.c_void_p(int(p)) for p in k_ptrs])
-        va = (C.c_void_p * L)(*[C.c_void_p(int(p)) for p in v_ptrs])
+        ka, va = self._plane_ptrs(k_ptrs, v_ptrs)
         check(lib().b200kv_import_peer_ptrs(self._h, peer_id, peer_device, ka, va,
                                              peer_block_stride or self.geom.stride,
                                              peer_n_blocks or self.geom.n_blocks),

@@ -140,12 +140,15 @@ struct Peer {
 
 struct Geometry {
   uint32_t L, H, D, elem, bs, C, planes;
+  uint32_t planes_per_layer;  // 2 (K, V), or 1 (MLA latent)
   uint32_t token_bytes;   // H*D*elem
   uint64_t slab_bytes;    // C*token_bytes (RAW) or C*H*D (FP8)
   uint64_t chunk_bytes;
-  uint64_t scales_off;    // FP8 only
+  uint64_t scales_off;    // FP8 K/V only
+  uint64_t scales_bytes;  // bytes at scales_off (0: the format has no separate scales area)
   uint32_t fmt_token_bytes;
   bool hnd;               // [H][bs][D] inside a block (B200KV_LAYOUT_HND)
+  bool mla;               // one latent plane per layer (B200KV_LAYOUT_MLA)
   uint32_t row_bytes;     // D*elem
 };
 
@@ -160,11 +163,16 @@ int make_geometry(const b200kv_engine_config* c, Geometry* g) {
   g->elem = c->elem_bytes;
   g->bs = c->block_tokens;
   g->C = c->chunk_tokens;
-  g->planes = 2u * g->L;
+  if (c->kv_layout != B200KV_LAYOUT_NHD && c->kv_layout != B200KV_LAYOUT_HND && c->kv_layout != B200KV_LAYOUT_MLA)
+    return B200KV_EINVAL;
+  g->hnd = c->kv_layout == B200KV_LAYOUT_HND;
+  g->mla = c->kv_layout == B200KV_LAYOUT_MLA;
+  if (g->mla && g->H != 1) return B200KV_EINVAL;  // the latent is per token, not per head
+  g->planes_per_layer = g->mla ? 1u : 2u;
+  g->planes = g->planes_per_layer * g->L;
   g->token_bytes = g->H * g->D * g->elem;
   g->row_bytes = g->D * g->elem;
-  if (c->kv_layout != B200KV_LAYOUT_NHD && c->kv_layout != B200KV_LAYOUT_HND) return B200KV_EINVAL;
-  g->hnd = c->kv_layout == B200KV_LAYOUT_HND;
+  g->scales_bytes = 0;
   if (g->token_bytes % 16) return B200KV_EINVAL;  // 16-byte vectors / bulk-copy granularity
   if (g->hnd && g->row_bytes % 16) return B200KV_EINVAL;
   if (c->format == B200KV_FMT_RAW) {
@@ -172,6 +180,13 @@ int make_geometry(const b200kv_engine_config* c, Geometry* g) {
     g->slab_bytes = static_cast<uint64_t>(g->C) * g->token_bytes;
     g->scales_off = 0;
     g->chunk_bytes = g->slab_bytes * g->planes;
+  } else if (c->format == B200KV_FMT_FP8 && g->mla) {
+    // per-token latent records (b200kv.h, B200KV_LAYOUT_MLA); the scales live inside each record
+    if (g->elem != 2 || g->D != kMlaDim) return B200KV_ENOTSUP;
+    g->fmt_token_bytes = kMlaRecordBytes;
+    g->slab_bytes = static_cast<uint64_t>(g->C) * g->fmt_token_bytes;
+    g->scales_off = 0;
+    g->chunk_bytes = (g->slab_bytes * g->planes + 255) / 256 * 256;
   } else if (c->format == B200KV_FMT_FP8) {
     if (g->elem != 2) return B200KV_ENOTSUP;  // source must be bf16
     if (g->hnd && (g->C / kCluster) % g->bs) return B200KV_ENOTSUP;  // a cluster window = whole tiles
@@ -181,10 +196,10 @@ int make_geometry(const b200kv_engine_config* c, Geometry* g) {
     g->fmt_token_bytes = g->token_bytes / 2;
     g->slab_bytes = static_cast<uint64_t>(g->C) * g->fmt_token_bytes;
     g->scales_off = g->slab_bytes * g->planes;
-    g->chunk_bytes = g->scales_off + static_cast<uint64_t>(g->planes) * g->H * sizeof(float);
-    g->chunk_bytes = (g->chunk_bytes + 255) / 256 * 256;
+    g->scales_bytes = static_cast<uint64_t>(g->planes) * g->H * sizeof(float);
+    g->chunk_bytes = (g->scales_off + g->scales_bytes + 255) / 256 * 256;
   } else if (c->format == B200KV_FMT_Q4) {
-    if (g->elem != 2) return B200KV_ENOTSUP;
+    if (g->elem != 2 || g->mla) return B200KV_ENOTSUP;
     if (g->D % 32) return B200KV_EINVAL;
     g->fmt_token_bytes = g->H * g->D / 2 + g->H * (g->D / 32) * 2;   // one token record of one plane
     g->slab_bytes = static_cast<uint64_t>(g->C) * g->fmt_token_bytes;
@@ -500,13 +515,27 @@ int launch_per_run(b200kv_ctx* ctx, CopyMode mode, const TableView& tv, size_t f
   return launched(ctx);
 }
 
+// FP8 latent records of an MLA engine, either direction, runs [f0, f0 + nf): one warp per (run, plane) unit.
+int launch_mla_fp8(b200kv_ctx* ctx, CopyMode mode, const TableView& tv, size_t f0, size_t nf, cudaStream_t s,
+                   uint32_t plane_begin, uint32_t n_planes) {
+  KernelArgs a = kernel_args(ctx, tv, f0, plane_begin, n_planes);
+  a.total_units = static_cast<uint32_t>(nf) * a.n_planes;
+  constexpr uint32_t warps = kMlaThreads / 32;
+  const uint32_t grid = std::min<uint32_t>((a.total_units + warps - 1) / warps, static_cast<uint32_t>(ctx->sm_count) * 8u);
+  if (grid == 0) return B200KV_OK;
+  if (mode == kStore) kv_mla_fp8_store_kernel<<<grid, kMlaThreads, 0, s>>>(a);
+  else kv_mla_fp8_load_kernel<<<grid, kMlaThreads, 0, s>>>(a);
+  return launched(ctx);
+}
+
 // Launches the kernels that move chunks [c0, c1) of table t, planes [pb, pb + np) (np == 0: every plane), in
-// direction `mode`.  A pull copies pages to pages whatever the chunk format.  The FP8 store always takes the
-// whole table.
+// direction `mode`.  A pull copies pages to pages whatever the chunk format.  The FP8 store of a K/V engine always
+// takes the whole table.
 int launch_op(b200kv_ctx* ctx, CopyMode mode, const OpTable& t, const TableView& tv, uint32_t c0, uint32_t c1,
               cudaStream_t s, uint32_t pb = 0, uint32_t np = 0, const Peer* peer = nullptr) {
   const size_t f0 = t.full_off[c0], nf = t.full_off[c1] - f0;
   const int fmt = mode == kPull ? B200KV_FMT_RAW : ctx->cfg.format;
+  if (fmt == B200KV_FMT_FP8 && ctx->g.mla) return launch_mla_fp8(ctx, mode, tv, f0, nf, s, pb, np);
   if (fmt == B200KV_FMT_FP8 && mode == kStore) return launch_fp8_store(ctx, t, tv, s);
   if (fmt != B200KV_FMT_RAW) return launch_per_run(ctx, mode, tv, f0, nf, s, pb, np);
   const size_t p0 = t.n_full() + t.part_off[c0], n_part = t.part_off[c1] - t.part_off[c0];
@@ -538,11 +567,10 @@ int copy_chunk_planes(b200kv_ctx* ctx, void* dst, const void* src, uint32_t n_to
     CU_TRY(cudaMemcpy2DAsync(d, g.slab_bytes, sp, g.slab_bytes, width, np, kind, s));
     moved = width * np;
   }
-  if (with_scales && !whole && ctx->cfg.format == B200KV_FMT_FP8) {
-    const size_t sb = static_cast<size_t>(g.planes) * g.H * sizeof(float);
+  if (with_scales && !whole && g.scales_bytes) {
     CU_TRY(cudaMemcpyAsync(static_cast<uint8_t*>(dst) + g.scales_off, static_cast<const uint8_t*>(src) + g.scales_off,
-                           sb, kind, s));
-    moved += sb;
+                           g.scales_bytes, kind, s));
+    moved += g.scales_bytes;
   }
   if (kind == cudaMemcpyDeviceToHost) ctx->stats.d2h_bytes += moved;
   else ctx->stats.h2d_bytes += moved;
@@ -753,7 +781,8 @@ static int engine_create_impl(const b200kv_engine_config* cfg, b200kv_pool* pool
   ctx->S = cfg->stages > 0 ? cfg->stages : env_int("B200KV_STAGES", 2);
   ctx->LAG = env_int("B200KV_LAG", ctx->S / 2);
   ctx->ctas_per_sm = cfg->ctas_per_sm > 0 ? cfg->ctas_per_sm : env_int("B200KV_CTAS_PER_SM", 1);
-  ctx->fp8_store3 = cfg->format == B200KV_FMT_FP8 && env_int("B200KV_FP8_STORE", 3) == 3 && fp8_store3_fits(g);
+  ctx->fp8_store3 = cfg->format == B200KV_FMT_FP8 && !g.mla && env_int("B200KV_FP8_STORE", 3) == 3 &&
+                    fp8_store3_fits(g);
   const uint32_t stage_max = static_cast<uint32_t>(env_int("B200KV_STAGE_KB", 32)) << 10;
   if (g.token_bytes > stage_max || stage_max > kStageMax * 2) return B200KV_ENOTSUP;
   ctx->piece_tokens = std::min<uint32_t>(g.bs, stage_max / g.token_bytes);
@@ -776,7 +805,7 @@ static int engine_create_impl(const b200kv_engine_config* cfg, b200kv_pool* pool
                          bulk_kernel<kPull>(ctx->S, ctx->LAG)})
       if (k) CU_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   }
-  if (cfg->format == B200KV_FMT_FP8) {
+  if (cfg->format == B200KV_FMT_FP8 && !g.mla) {
     CU_TRY(cudaFuncSetAttribute(kv_fp8_store3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 kS3Stages * kS3MaxUnitBytes));
     CU_TRY(cudaFuncSetAttribute(kv_fp8_store_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
@@ -879,7 +908,7 @@ extern "C" int b200kv_engine_destroy(b200kv_ctx* ctx) {
 // its cluster kernel.
 static void build_tensor_maps(b200kv_ctx* ctx, const std::vector<uint64_t>& bases) {
   const Geometry& g = ctx->g;
-  if (ctx->cfg.format != B200KV_FMT_FP8 || g.elem != 2 || g.hnd) { ctx->tmap_status = "not needed"; return; }
+  if (ctx->cfg.format != B200KV_FMT_FP8 || g.elem != 2 || g.hnd || g.mla) { ctx->tmap_status = "not needed"; return; }
   typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -924,18 +953,19 @@ static void build_tensor_maps(b200kv_ctx* ctx, const std::vector<uint64_t>& base
 
 extern "C" int b200kv_register_kv(b200kv_ctx* ctx, const void* const* k_ptrs,
                                   const void* const* v_ptrs) {
-  if (!ctx || !k_ptrs || !v_ptrs) return B200KV_EINVAL;
+  const uint32_t ppl = ctx ? ctx->g.planes_per_layer : 0;
+  if (!ctx || !k_ptrs || (ppl == 2) != (v_ptrs != nullptr)) return B200KV_EINVAL;   // MLA: v_ptrs NULL
   DeviceGuard dg(ctx->cfg.device);
   std::lock_guard<std::mutex> lk(ctx->mu);
   std::vector<uint64_t> h(ctx->g.planes);
   ctx->h_k.assign(k_ptrs, k_ptrs + ctx->g.L);
-  ctx->h_v.assign(v_ptrs, v_ptrs + ctx->g.L);
+  if (v_ptrs) ctx->h_v.assign(v_ptrs, v_ptrs + ctx->g.L);
   for (uint32_t l = 0; l < ctx->g.L; ++l) {
-    const uint64_t k = reinterpret_cast<uint64_t>(k_ptrs[l]);
-    const uint64_t v = reinterpret_cast<uint64_t>(v_ptrs[l]);
-    if (!k || !v || (k % 16) || (v % 16)) return B200KV_EINVAL;
-    h[2 * l] = k;
-    h[2 * l + 1] = v;
+    for (uint32_t kv = 0; kv < ppl; ++kv) {
+      const uint64_t p = reinterpret_cast<uint64_t>(kv ? v_ptrs[l] : k_ptrs[l]);
+      if (!p || p % 16) return B200KV_EINVAL;
+      h[ppl * l + kv] = p;
+    }
   }
   CU_TRY(cudaMemcpy(ctx->d_bases, h.data(), sizeof(uint64_t) * h.size(), cudaMemcpyHostToDevice));
   build_tensor_maps(ctx, h);
@@ -1258,8 +1288,8 @@ static int load_impl(b200kv_ctx* ctx, const uint64_t* keys, const int32_t* chunk
       op->layers_per_group = layers_per_group;
       op->group_ev.resize(n_groups, nullptr);
       for (uint32_t gi = 0; gi < n_groups; ++gi) {
-        const uint32_t pb = 2 * gi * G;
-        const uint32_t np = std::min<uint32_t>(2 * G, g.planes - pb);
+        const uint32_t pb = g.planes_per_layer * gi * G;
+        const uint32_t np = std::min<uint32_t>(g.planes_per_layer * G, g.planes - pb);
         for (uint32_t i = 0; i < nb; ++i) {
           const Todo& t = todo[b0 + i];
           rc = copy_chunk_planes(ctx, reinterpret_cast<void*>(addrs[i]), b200kv_pool_slot_ptr(ctx->pool, t.slot),
@@ -1456,12 +1486,12 @@ extern "C" int b200kv_export_ipc(b200kv_ctx* ctx, b200kv_ipc_desc* descs_out, in
   if (!fn || qr != cudaDriverEntryPointSuccess) return B200KV_ENODEV;
   GetRange get_range = reinterpret_cast<GetRange>(fn);
   for (uint32_t l = 0; l < ctx->g.L; ++l) {
-    for (int kv = 0; kv < 2; ++kv) {
+    for (uint32_t kv = 0; kv < ctx->g.planes_per_layer; ++kv) {
       const void* p = kv ? ctx->h_v[l] : ctx->h_k[l];
       CUdeviceptr base = 0;
       size_t size = 0;
       if (get_range(&base, &size, reinterpret_cast<CUdeviceptr>(p)) != CUDA_SUCCESS) return B200KV_ENODEV;
-      b200kv_ipc_desc& d = descs_out[kv * ctx->g.L + l];  // K planes then V planes
+      b200kv_ipc_desc& d = descs_out[kv * ctx->g.L + l];  // K planes then V planes (MLA: latent planes)
       std::memset(&d, 0, sizeof(d));
       cudaIpcMemHandle_t h;
       CU_TRY(cudaIpcGetMemHandle(&h, reinterpret_cast<void*>(base)));
@@ -1502,8 +1532,9 @@ extern "C" int b200kv_import_peer(b200kv_ctx* ctx, int32_t peer_id, int32_t peer
   std::vector<std::pair<std::string, void*>> seen;
   std::vector<void*> opened;
   std::vector<uint64_t> bases(ctx->g.planes);
+  const uint32_t ppl = ctx->g.planes_per_layer;
   for (uint32_t l = 0; l < ctx->g.L; ++l) {
-    for (int kv = 0; kv < 2; ++kv) {
+    for (uint32_t kv = 0; kv < ppl; ++kv) {
       const b200kv_ipc_desc& d = descs[kv * ctx->g.L + l];
       const std::string key(reinterpret_cast<const char*>(d.handle), 64);
       void* base = nullptr;
@@ -1516,7 +1547,7 @@ extern "C" int b200kv_import_peer(b200kv_ctx* ctx, int32_t peer_id, int32_t peer
         seen.emplace_back(key, base);
         opened.push_back(base);
       }
-      bases[2 * l + kv] = reinterpret_cast<uint64_t>(base) + d.offset;
+      bases[ppl * l + kv] = reinterpret_cast<uint64_t>(base) + d.offset;
     }
   }
   return install_peer(ctx, peer_id, peer_device, bases, peer_block_stride_bytes, peer_n_blocks,
@@ -1526,7 +1557,9 @@ extern "C" int b200kv_import_peer(b200kv_ctx* ctx, int32_t peer_id, int32_t peer
 extern "C" int b200kv_import_peer_ptrs(b200kv_ctx* ctx, int32_t peer_id, int32_t peer_device,
                                        const void* const* k_ptrs, const void* const* v_ptrs,
                                        uint64_t peer_block_stride_bytes, uint64_t peer_n_blocks) {
-  if (!ctx || !k_ptrs || !v_ptrs || peer_id < 0 || peer_id >= kMaxPeers) return B200KV_EINVAL;
+  if (!ctx || !k_ptrs || (ctx->g.planes_per_layer == 2) != (v_ptrs != nullptr) || peer_id < 0 ||
+      peer_id >= kMaxPeers)
+    return B200KV_EINVAL;
   if (peer_n_blocks == 0 || peer_n_blocks * ctx->g.bs > 0x7fffffffull) return B200KV_EINVAL;
   DeviceGuard dg(ctx->cfg.device);
   std::lock_guard<std::mutex> lk(ctx->mu);
@@ -1541,12 +1574,13 @@ extern "C" int b200kv_import_peer_ptrs(b200kv_ctx* ctx, int32_t peer_id, int32_t
     }
     cudaGetLastError();
   }
+  const uint32_t ppl = ctx->g.planes_per_layer;
   std::vector<uint64_t> bases(ctx->g.planes);
   for (uint32_t l = 0; l < ctx->g.L; ++l) {
-    bases[2 * l] = reinterpret_cast<uint64_t>(k_ptrs[l]);
-    bases[2 * l + 1] = reinterpret_cast<uint64_t>(v_ptrs[l]);
-    if (!bases[2 * l] || !bases[2 * l + 1] || bases[2 * l] % 16 || bases[2 * l + 1] % 16)
-      return B200KV_EINVAL;
+    for (uint32_t kv = 0; kv < ppl; ++kv) {
+      bases[ppl * l + kv] = reinterpret_cast<uint64_t>(kv ? v_ptrs[l] : k_ptrs[l]);
+      if (!bases[ppl * l + kv] || bases[ppl * l + kv] % 16) return B200KV_EINVAL;
+    }
   }
   return install_peer(ctx, peer_id, peer_device, bases, peer_block_stride_bytes, peer_n_blocks, {});
 }

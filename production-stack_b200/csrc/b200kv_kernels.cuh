@@ -29,6 +29,8 @@
 //   kv_fp8_load_kernel     bulk-load e4m3 piece -> dequantise -> 16-byte stores into the pages.
 //   kv_q4_store_kernel /   group-wise 4-bit chunks: one 16-byte vector per thread, a group is a quad
 //   kv_q4_load_kernel      of lanes.
+//   kv_mla_fp8_store_kernel /  FP8 latent records of MLA engines: one warp per (token, plane), a group of
+//   kv_mla_fp8_load_kernel     128 elements is 16 lanes; no shared memory.
 //
 // Every kernel takes one KernelArgs, filled by kernel_args() in b200kv_engine.cu.
 #pragma once
@@ -43,7 +45,7 @@
 namespace b200kv {
 
 struct PagedSide {
-  const uint64_t* bases;  // device array [2*L]: K plane of layer l at [2l], V plane at [2l+1]
+  const uint64_t* bases;  // device array [2*L]: K plane of layer l at [2l], V plane at [2l+1]; MLA: [L] latent planes
   uint64_t block_stride;  // bytes between consecutive blocks of one plane
   uint32_t block_tokens;
   uint32_t token_bytes;   // H*D*elem (NHD: one token's heads are contiguous)
@@ -973,6 +975,109 @@ __global__ void __launch_bounds__(256) kv_q4_load_kernel(const KernelArgs p) {
         }
         st_na_v4(reinterpret_cast<void*>(q4_src_addr(p, plane, static_cast<uint32_t>(run.a) + tt[j], vv[j])),
                  make_uint4(o[0], o[1], o[2], o[3]));
+      }
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// FP8 latent records of an MLA engine (B200KV_LAYOUT_MLA + B200KV_FMT_FP8; spec: tests/mla_oracle.py).
+// A bf16 page row is 576 elements = 72 16-byte vectors: latent vectors 0..63 (group g = vectors
+// [16g, 16g+16)), RoPE vectors 64..71.  A record is [512 e4m3 codes][4 fp32 scales][64 bf16 RoPE].
+// One warp per (token, plane): lane l holds latent vectors l and l+32, so lanes 0-15 see groups 0 and 2 and
+// lanes 16-31 groups 1 and 3, and each half reduces both of its groups at once with four shuffles of two
+// packed bf16 magnitudes.  Lane l writes 8 code bytes per vector (256 contiguous bytes per warp and vector),
+// lane 0 writes the four scales as one 16-byte store, lanes 0-7 move the RoPE vectors.  No shared memory.
+// A unit is one (run, plane): total_units = n_runs * n_planes; the warp walks the run kMlaTokens tokens at a
+// time with all of their loads issued first.
+// ---------------------------------------------------------------------------------------------
+constexpr uint32_t kMlaDim = 576;            // kv_lora_rank 512 + qk_rope_head_dim 64
+constexpr uint32_t kMlaRecordBytes = 656;    // 41 * 16
+constexpr uint32_t kMlaScalesOff = 512;
+constexpr uint32_t kMlaRopeOff = 528;        // 33 * 16
+constexpr int kMlaThreads = 256;
+constexpr int kMlaTokens = 4;
+
+// scale = fl32(absmax / 448), inv = fl32(448 / absmax), both 1 when absmax is 0 (m = bf16 bits of absmax)
+__device__ __forceinline__ float mla_scale(uint32_t m) { return m ? __fdiv_rn(__uint_as_float(m << 16), 448.0f) : 1.0f; }
+__device__ __forceinline__ float mla_inv(uint32_t m) { return m ? __fdiv_rn(448.0f, __uint_as_float(m << 16)) : 1.0f; }
+
+__device__ __forceinline__ uint32_t absmax_vec(const uint4& v) {
+  const uint32_t acc = absmax_u16x2(absmax_u16x2(absmax_u16x2(absmax_u16x2(0u, v.x), v.y), v.z), v.w);
+  return max(acc & 0xffffu, acc >> 16);
+}
+
+__global__ void __launch_bounds__(kMlaThreads) kv_mla_fp8_store_kernel(const KernelArgs p) {
+  const uint32_t lane = threadIdx.x & 31u;
+  const uint32_t n_warps = gridDim.x * (kMlaThreads / 32);
+  for (uint32_t ui = blockIdx.x * (kMlaThreads / 32) + threadIdx.x / 32; ui < p.total_units; ui += n_warps) {
+    const uint32_t plane = p.plane_begin + ui % p.n_planes;
+    const Run run = p.runs[ui / p.n_planes];
+    for (int32_t j = 0; j < run.n; j += kMlaTokens) {
+      uint4 a[kMlaTokens], b[kMlaTokens], r[kMlaTokens];
+#pragma unroll
+      for (int k = 0; k < kMlaTokens; ++k) {   // every load of the step first
+        r[k] = a[k] = b[k] = make_uint4(0, 0, 0, 0);
+        if (j + k >= run.n) continue;
+        const uint8_t* row = reinterpret_cast<const uint8_t*>(paged_addr(p.paged, plane, static_cast<uint32_t>(run.a + j + k)));
+        a[k] = ld_nc_v4(row + 16 * lane);
+        b[k] = ld_nc_v4(row + 512 + 16 * lane);
+        if (lane < 8) r[k] = ld_nc_v4(row + 1024 + 16 * lane);
+      }
+#pragma unroll
+      for (int k = 0; k < kMlaTokens; ++k) {
+        if (j + k >= run.n) break;   // uniform over the warp
+        uint32_t m = absmax_vec(a[k]) | (absmax_vec(b[k]) << 16);   // lo: group lane/16, hi: group 2 + lane/16
+        m = __vmaxu2(m, __shfl_xor_sync(0xffffffffu, m, 1));
+        m = __vmaxu2(m, __shfl_xor_sync(0xffffffffu, m, 2));
+        m = __vmaxu2(m, __shfl_xor_sync(0xffffffffu, m, 4));
+        m = __vmaxu2(m, __shfl_xor_sync(0xffffffffu, m, 8));
+        const uint32_t other = __shfl_xor_sync(0xffffffffu, m, 16);
+        uint8_t* rec = reinterpret_cast<uint8_t*>(chunk_addr(p.chunk, plane, static_cast<uint32_t>(run.b + j + k)));
+        st_na_v2(rec + 8 * lane, quant8(a[k], mla_inv(m & 0xffffu)));
+        st_na_v2(rec + 256 + 8 * lane, quant8(b[k], mla_inv(m >> 16)));
+        if (lane == 0) {
+          const float4 s = make_float4(mla_scale(m & 0xffffu), mla_scale(other & 0xffffu), mla_scale(m >> 16),
+                                       mla_scale(other >> 16));
+          st_na_v4(rec + kMlaScalesOff, *reinterpret_cast<const uint4*>(&s));
+        }
+        if (lane < 8) st_na_v4(rec + kMlaRopeOff + 16 * lane, r[k]);
+      }
+    }
+  }
+}
+
+__global__ void __launch_bounds__(kMlaThreads) kv_mla_fp8_load_kernel(const KernelArgs p) {
+  const uint32_t lane = threadIdx.x & 31u;
+  const uint32_t half = lane >> 4;
+  const uint32_t n_warps = gridDim.x * (kMlaThreads / 32);
+  for (uint32_t ui = blockIdx.x * (kMlaThreads / 32) + threadIdx.x / 32; ui < p.total_units; ui += n_warps) {
+    const uint32_t plane = p.plane_begin + ui % p.n_planes;
+    const Run run = p.runs[ui / p.n_planes];
+    for (int32_t j = 0; j < run.n; j += kMlaTokens) {
+      uint2 qa[kMlaTokens], qb[kMlaTokens];
+      float sa[kMlaTokens], sb[kMlaTokens];
+      uint4 r[kMlaTokens];
+#pragma unroll
+      for (int k = 0; k < kMlaTokens; ++k) {   // every load of the step first
+        qa[k] = qb[k] = make_uint2(0, 0);
+        sa[k] = sb[k] = 0.0f;
+        r[k] = make_uint4(0, 0, 0, 0);
+        if (j + k >= run.n) continue;
+        const uint8_t* rec = reinterpret_cast<const uint8_t*>(chunk_addr(p.chunk, plane, static_cast<uint32_t>(run.b + j + k)));
+        qa[k] = __ldg(reinterpret_cast<const uint2*>(rec + 8 * lane));
+        qb[k] = __ldg(reinterpret_cast<const uint2*>(rec + 256 + 8 * lane));
+        sa[k] = __ldg(reinterpret_cast<const float*>(rec + kMlaScalesOff) + half);
+        sb[k] = __ldg(reinterpret_cast<const float*>(rec + kMlaScalesOff) + 2 + half);
+        if (lane < 8) r[k] = ld_nc_v4(rec + kMlaRopeOff + 16 * lane);
+      }
+#pragma unroll
+      for (int k = 0; k < kMlaTokens; ++k) {
+        if (j + k >= run.n) break;
+        uint8_t* row = reinterpret_cast<uint8_t*>(paged_addr(p.paged, plane, static_cast<uint32_t>(run.a + j + k)));
+        st_na_v4(row + 16 * lane, dequant8(qa[k], sa[k]));
+        st_na_v4(row + 512 + 16 * lane, dequant8(qb[k], sb[k]));
+        if (lane < 8) st_na_v4(row + 1024 + 16 * lane, r[k]);
       }
     }
   }
