@@ -54,14 +54,23 @@ extern "C" {
  *        (vllm_v1_adapter.py:471-477).  Bit-exact round trip.
  * FP8  : (L, 2, C, H, D) bytes of e4m3fn followed by (L, 2, H) fp32 scales; one scale per
  *        (chunk, layer, K/V, head) = absmax/448 (SURVEY.md §8c tolerance).  Source dtype
- *        must be bf16.  Stands in for LMCACHE_REMOTE_SERDE=cachegen's lossy codec
+ *        bf16, or fp16 after b200kv_set_cache_dtype; decoding rounds once to the source dtype.
+ *        Stands in for LMCACHE_REMOTE_SERDE=cachegen's lossy codec
  *        (helm/templates/deployment-vllm-multi.yaml:341-344).                              */
 #define B200KV_FMT_RAW 0
 #define B200KV_FMT_FP8 1
 /* Q4 (experimental): group-wise 4-bit — per (token, head) groups of 32 elements, bf16 scale = absmax/7,
  * two's-complement nibbles; a stored token of one plane is [H*D/2 codes][H*D/32 scales] (4.5 bits per
- * element).  Specified by oracle/kv_oracle.py q4_pack_chunk.  Source dtype bf16, D % 32 == 0.        */
+ * element).  Specified by oracle/kv_oracle.py q4_pack_chunk (tests/fp16_oracle.py for fp16 caches).
+ * Source dtype bf16 or fp16 (the scales stay bf16 for both), D % 32 == 0.                         */
 #define B200KV_FMT_Q4 2
+
+/* ---- element type of the paged cache (b200kv_set_cache_dtype) ---------------------------- */
+/* The lossy formats decode the cache's 16-bit elements, so they must know which type they are.  RAW moves
+ * bytes and needs no type, but the type is part of every chunk's format tag in either case, so bf16 and
+ * fp16 chunks never mix in a pool, a device tier or a cache server.                          */
+#define B200KV_DTYPE_BF16 0   /* default */
+#define B200KV_DTYPE_FP16 1
 
 /* ---- order inside one (block, K|V) tile of the paged cache ------------------------------ */
 /* NHD: [block_tokens][H][D] (FlashAttention default, vllm/v1/attention/backends/flash_attn.py:
@@ -80,9 +89,10 @@ extern "C" {
  *      (v1/attention/backends/mla/flashmla_sparse.py:68-79):
  *        [0, 512)    e4m3 codes of latent elements 0..511
  *        [512, 528)  4 fp32 scales, scale g = absmax(elements [128g, 128g+128)) / 448 (1 if absmax is 0)
- *        [528, 656)  RoPE elements 512..575, bf16 bits copied verbatim
+ *        [528, 656)  RoPE elements 512..575, the cache's 16-bit bits copied verbatim
  *      A chunk is L slabs of C records (no separate scales area), rounded up to 256 bytes.  Needs a bf16
- *      cache and D == 576; Q4 is not offered on MLA (-ENOTSUP).                                  */
+ *      or fp16 cache and D == 576; Q4 is not offered on MLA (-ENOTSUP).  In an fp16 cache the RoPE part
+ *      is fp16 bits, where vLLM's fp8_ds_mla has bf16; such chunks carry the fp16 format tag.      */
 #define B200KV_LAYOUT_MLA 2
 
 /* ---- kernel variants (both are CUDA; selectable for A/B measurement) ------------------- */
@@ -236,6 +246,10 @@ typedef struct b200kv_engine_stats {
 /* Engine construction (stands in for _init_lmcache_engine, vllm_v1_adapter.py:433-558).
  * `pool` may be NULL for an engine used only through gather/scatter/peer_pull.             */
 int b200kv_engine_create(const b200kv_engine_config* cfg, b200kv_pool* pool, b200kv_ctx** out);
+/* Element type of the cache, B200KV_DTYPE_* (bf16 until set).  Legal between b200kv_engine_create and
+ * b200kv_register_kv: -EBUSY after registration.  FP16 needs elem_bytes == 2, else -EINVAL.  A function
+ * rather than a config field, so the v1 config layout and every existing binding stay valid.     */
+int b200kv_set_cache_dtype(b200kv_ctx* ctx, int32_t dtype);
 /* What the engine did about host-page placement when it pinned the pool (numa_policy above), as text
  * for logs and bench output, e.g. "mbind preferred node 1".                                  */
 int b200kv_engine_numa_placement(b200kv_ctx* ctx, char* buf, uint64_t n);

@@ -25,7 +25,7 @@ from vllm.distributed.kv_transfer.kv_connector.v1.base import (KVConnectorBase_V
 from . import _lib
 from .adapter import ReqMeta, SchedulerState, WorkerState, request_identity
 from .config import B200KVConfig
-from .engine import KVEngine, KVGeometry, KVPool, paged_layout_of, xxh64
+from .engine import KVEngine, KVGeometry, KVPool, dtype_code, paged_layout_of, xxh64
 from .pd import PDMeta, PDScheduler, PDWorker, first_group, publish_ipc, unpublish_ipc
 
 if TYPE_CHECKING:
@@ -73,18 +73,24 @@ def geometry_from_vllm(vllm_config, cfg: B200KVConfig, n_blocks: int = 1) -> KVG
     """LMCache's kv_shape = (num_layer, 2, chunk, num_kv_head, head_size)
     (vllm_v1_adapter.py:471-477), derivable in both roles from the vLLM config alone.  An MLA model
     (model_config.use_mla) has one latent plane per layer: (num_layer, 1, chunk, 1, head_size)
-    (vllm_v1_adapter.py:463-477)."""
+    (vllm_v1_adapter.py:463-477).  The cache's element type: the model's with cache_dtype "auto",
+    named by "float16" / "bfloat16"; every other cache dtype (fp8*, ...) keeps bf16, which only RAW reads."""
     mc, pc, cc = vllm_config.model_config, vllm_config.parallel_config, vllm_config.cache_config
     dt = str(cc.cache_dtype)
+    dtype = _lib.DTYPE_BF16
     if dt in ("auto", "None"):
         elem = torch.empty((), dtype=mc.dtype).element_size()
+        if mc.dtype == torch.float16:
+            dtype = _lib.DTYPE_FP16
     else:
         elem = 1 if "fp8" in dt else 2
+        if dt == "float16":
+            dtype = _lib.DTYPE_FP16
     mla = bool(getattr(mc, "use_mla", False))
     return KVGeometry(n_layers=mc.get_num_layers(pc), n_kv_heads=1 if mla else mc.get_num_kv_heads(pc),
                       head_dim=mc.get_head_size(), n_blocks=n_blocks, block_tokens=cc.block_size,
                       chunk_tokens=cfg.chunk_size, elem_bytes=elem, block_stride_bytes=0, fmt=cfg.fmt,
-                      layout=_lib.LAYOUT_MLA if mla else _lib.LAYOUT_NHD)
+                      layout=_lib.LAYOUT_MLA if mla else _lib.LAYOUT_NHD, dtype=dtype)
 
 
 def owner_tag_of(instance_id: str) -> int:
@@ -241,10 +247,12 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
         geom = KVGeometry(n_layers=len(tensors), n_kv_heads=h, head_dim=d, n_blocks=nb,
                           block_tokens=self._block_size, chunk_tokens=self._chunk,
                           elem_bytes=t0.element_size(), block_stride_bytes=stride, fmt=self.cfg.fmt,
-                          layout=tile_layout)
+                          layout=tile_layout, dtype=dtype_code(t0.dtype) or _lib.DTYPE_BF16)
         if geom.chunk_bytes != geom0.chunk_bytes:
             raise ValueError("KV cache tensors do not match the model geometry the pool was sized for "
                              f"({geom.chunk_bytes} vs {geom0.chunk_bytes} bytes per chunk)")
+        if geom.dtype != geom0.dtype:   # the key seed is derived from the vLLM config's type
+            raise ValueError(f"KV cache dtype {t0.dtype} differs from the one the vLLM config implies")
         rank = getattr(self._vllm_config.parallel_config, "rank", 0)
         self._rank = rank
         self._engine = KVEngine(geom, self._pool, device=t0.device.index or 0,
@@ -262,7 +270,7 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
                                    stores=not geom.mla or self._tp_rank() == 0)   # MLA: rank 0 stores for all ranks
         if self.cfg.device_tier_gb > 0:
             from .device_tier import LocalTier, TierSet
-            fmt_tag = self.cfg.fmt | (tile_layout << 8)
+            fmt_tag = geom.fmt_tag
             try:
                 n_slots = max(1, int(self.cfg.device_tier_gb * (1 << 30)) // geom.chunk_bytes)
                 self._worker.tiers = TierSet(self._engine_id, geom.chunk_bytes, fmt_tag, importer=self._engine.tier_import)

@@ -59,6 +59,12 @@ def xxh64(data: bytes, seed: int = 0) -> int:
                                   C.c_uint64(seed)))
 
 
+def dtype_code(torch_dtype) -> int | None:
+    """torch dtype of a cache -> DTYPE_BF16 / DTYPE_FP16; None for every other type."""
+    name = str(torch_dtype)
+    return {"torch.bfloat16": _lib.DTYPE_BF16, "torch.float16": _lib.DTYPE_FP16}.get(name)
+
+
 @dataclass(frozen=True)
 class KVGeometry:
     """Model / cache geometry (LMCache's kv_shape = (L, 2, chunk, H, D),
@@ -73,6 +79,17 @@ class KVGeometry:
     block_stride_bytes: int = 0   # 0 -> dense (block_tokens * H * D * elem)
     fmt: int = FMT_RAW
     layout: int = 0               # LAYOUT_NHD / LAYOUT_HND inside a block, or LAYOUT_MLA
+    dtype: int = _lib.DTYPE_BF16  # element type of a 16-bit cache: DTYPE_BF16 or DTYPE_FP16 (b200kv_set_cache_dtype)
+
+    @property
+    def fp16(self) -> bool:
+        return self.dtype == _lib.DTYPE_FP16
+
+    @property
+    def fmt_tag(self) -> int:
+        """The format tag the engine records with every chunk (pool_fmt in b200kv_engine.cu): format, tile order
+        and cache element type.  bf16 tags are format | layout << 8, as before the element type was added."""
+        return self.fmt | (self.layout << 8) | (self.dtype << 16)
 
     @property
     def token_bytes(self) -> int:
@@ -95,12 +112,15 @@ class KVGeometry:
         """Namespace for chunk keys: same role as LMCache's CacheEngineKey(fmt, model, world_size,
         worker_id, ...) — chunks of different models / shards / formats never alias.  An MLA latent is
         the same on every tensor-parallel rank, so its namespace keeps only the pipeline stage
-        (rank // world_size) of the rank: one stored copy serves every rank of the stage."""
+        (rank // world_size) of the rank: one stored copy serves every rank of the stage.  An fp16 cache
+        appends "|fp16", so its chunks (RAW included) never alias a bf16 replica's; bf16 seeds are unchanged."""
         if self.mla:
             rank //= max(world_size, 1)
         tag = f"{model}|{world_size}|{rank}|{self.n_layers}|{self.n_kv_heads}|{self.head_dim}|" \
-              f"{self.elem_bytes}|{self.chunk_tokens}|{self.fmt}|{self.layout}".encode()
-        return xxh64(tag, DEFAULT_SEED)
+              f"{self.elem_bytes}|{self.chunk_tokens}|{self.fmt}|{self.layout}"
+        if self.fp16:
+            tag += "|fp16"
+        return xxh64(tag.encode(), DEFAULT_SEED)
 
     def to_c(self, device: int, staging_bytes: int, owner: int, variant: int, stages: int,
              ctas_per_sm: int, numa_policy: int = 0) -> _lib.EngineConfig:
@@ -316,6 +336,12 @@ class KVEngine:
               "b200kv_engine_create")
         self._h = h
         self._kv_refs = None
+        if geom.fp16:
+            self.set_cache_dtype(_lib.DTYPE_FP16)
+
+    def set_cache_dtype(self, dtype: int):
+        """b200kv_set_cache_dtype: legal before registration only (-EBUSY after)."""
+        check(lib().b200kv_set_cache_dtype(self._h, dtype), "b200kv_set_cache_dtype")
 
     # ---- registration ---------------------------------------------------------------------
     def _plane_ptrs(self, k_ptrs, v_ptrs):
@@ -344,6 +370,11 @@ class KVEngine:
                     or nb < self.geom.n_blocks or t.element_size() != self.geom.elem_bytes \
                     or tl != self.geom.layout:
                 raise ValueError("KV cache tensor does not match the engine geometry")
+            if self.geom.fmt != FMT_RAW and dtype_code(t.dtype) != self.geom.dtype:
+                # the lossy kernels decode the elements: fp16 bits read as bf16 (or the reverse) would be stored
+                # and loaded as wrong values without any error
+                raise ValueError(f"KV cache dtype {t.dtype} does not match the engine's cache dtype "
+                                 f"({'float16' if self.geom.fp16 else 'bfloat16'})")
             ks.append(k)
             vs.append(v)
         self._kv_refs = tensors  # keep the storage alive

@@ -33,6 +33,8 @@ from dataclasses import dataclass, field
 
 import numpy as np
 
+from ._lib import DTYPE_BF16
+
 SHM_DIR = os.environ.get("B200KV_SHM_DIR", "/dev/shm")
 
 
@@ -71,12 +73,17 @@ def trace(event: str, **kw):
 # ------------------------------------------------------------------------------------------------
 # publication of a replica's cache (worker role, after register_kv_caches)
 # ------------------------------------------------------------------------------------------------
+def _dtype_of(geom) -> int:
+    """The cache element type of a geometry (KVGeometry.dtype; bf16 for a geometry without one)."""
+    return int(getattr(geom, "dtype", DTYPE_BF16))
+
+
 def publish_ipc(engine_id: str, engine, device: int, rank: int = 0, tp_size: int = 1) -> str:
     g = engine.geom
     doc = {"engine_id": engine_id, "device": device, "pid": os.getpid(), "rank": rank, "tp_size": tp_size,
            "n_blocks": g.n_blocks,
            "block_stride": g.stride, "n_layers": g.n_layers, "n_kv_heads": g.n_kv_heads, "head_dim": g.head_dim,
-           "block_tokens": g.block_tokens, "elem_bytes": g.elem_bytes, "layout": g.layout,
+           "block_tokens": g.block_tokens, "elem_bytes": g.elem_bytes, "layout": g.layout, "dtype": _dtype_of(g),
            "descs": base64.b64encode(engine.export_ipc()).decode()}
     path = ipc_path(engine_id, rank)
     tmp = path + f".{os.getpid()}.tmp"
@@ -125,8 +132,10 @@ class PeerResolver:
             raise ValueError(f"peer {remote_engine_id}: tensor-parallel layout {doc.get('rank')}/{doc.get('tp_size')} "
                              f"differs from local {self.rank}/{self.tp_size}")
         g = self.engine.geom
+        doc.setdefault("dtype", DTYPE_BF16)   # documents published before the field are bf16 caches
         for k, mine in (("n_layers", g.n_layers), ("n_kv_heads", g.n_kv_heads), ("head_dim", g.head_dim),
-                        ("block_tokens", g.block_tokens), ("elem_bytes", g.elem_bytes), ("layout", g.layout)):
+                        ("block_tokens", g.block_tokens), ("elem_bytes", g.elem_bytes), ("layout", g.layout),
+                        ("dtype", _dtype_of(g))):
             if doc[k] != mine:
                 raise ValueError(f"peer {remote_engine_id}: {k}={doc[k]} differs from local {mine}")
         pid = len(self.ids)

@@ -150,6 +150,7 @@ struct Geometry {
   bool hnd;               // [H][bs][D] inside a block (B200KV_LAYOUT_HND)
   bool mla;               // one latent plane per layer (B200KV_LAYOUT_MLA)
   uint32_t row_bytes;     // D*elem
+  uint32_t dtype;         // B200KV_DTYPE_*: element type of the cache (b200kv_set_cache_dtype; bf16 by default)
 };
 
 int make_geometry(const b200kv_engine_config* c, Geometry* g) {
@@ -172,6 +173,7 @@ int make_geometry(const b200kv_engine_config* c, Geometry* g) {
   g->planes = g->planes_per_layer * g->L;
   g->token_bytes = g->H * g->D * g->elem;
   g->row_bytes = g->D * g->elem;
+  g->dtype = B200KV_DTYPE_BF16;
   g->scales_bytes = 0;
   if (g->token_bytes % 16) return B200KV_EINVAL;  // 16-byte vectors / bulk-copy granularity
   if (g->hnd && g->row_bytes % 16) return B200KV_EINVAL;
@@ -188,7 +190,7 @@ int make_geometry(const b200kv_engine_config* c, Geometry* g) {
     g->scales_off = 0;
     g->chunk_bytes = (g->slab_bytes * g->planes + 255) / 256 * 256;
   } else if (c->format == B200KV_FMT_FP8) {
-    if (g->elem != 2) return B200KV_ENOTSUP;  // source must be bf16
+    if (g->elem != 2) return B200KV_ENOTSUP;  // source must be bf16 or fp16
     if (g->hnd && (g->C / kCluster) % g->bs) return B200KV_ENOTSUP;  // a cluster window = whole tiles
     if (g->H > kMaxHeads) return B200KV_ENOTSUP;
     if (g->C % kCluster) return B200KV_EINVAL;
@@ -405,10 +407,11 @@ BulkKernel bulk_kernel(int S, int LAG) {
   }
 }
 
-// format tag recorded with a chunk: a pool shared by engines of different tile order or codec
-// never hands one engine's bytes to another
+// format tag recorded with a chunk: a pool shared by engines of different tile order, codec or cache element
+// type never hands one engine's bytes to another (bf16 engines keep the tags they had before the dtype field)
 uint32_t pool_fmt(const b200kv_ctx* ctx) {
-  return static_cast<uint32_t>(ctx->cfg.format) | (static_cast<uint32_t>(ctx->cfg.kv_layout) << 8);
+  return static_cast<uint32_t>(ctx->cfg.format) | (static_cast<uint32_t>(ctx->cfg.kv_layout) << 8) |
+         (ctx->g.dtype << 16);
 }
 
 PagedSide local_side(const b200kv_ctx* ctx) {
@@ -479,7 +482,8 @@ int launch_copy_runs(b200kv_ctx* ctx, const TableView& tv, size_t f0, size_t nf,
 
 // FP8 store of every chunk of the table; chunks of several requests may be partial anywhere.  The persistent
 // kernel takes the table when the engine allows it (fp8_store3) and every chunk is whole, block-aligned runs; the
-// cluster kernel takes every other table.
+// cluster kernel takes every other table.  DT: the cache's element type (the lossy launchers are built per type).
+template <int DT>
 int launch_fp8_store(b200kv_ctx* ctx, const OpTable& t, const TableView& tv, cudaStream_t s) {
   const Geometry& g = ctx->g;
   KernelArgs a = kernel_args(ctx, tv, 0, 0, 0);
@@ -488,18 +492,19 @@ int launch_fp8_store(b200kv_ctx* ctx, const OpTable& t, const TableView& tv, cud
     const size_t smem = static_cast<size_t>(kS3Stages) * g.C * g.row_bytes;
     const uint32_t grid = std::min<uint32_t>(a.total_units, static_cast<uint32_t>(ctx->sm_count));
     if (grid == 0) return B200KV_OK;
-    kv_fp8_store3_kernel<<<grid, kS3Threads, smem, s>>>(a, g.hnd ? nullptr : ctx->d_tmaps);
+    kv_fp8_store3_kernel<DT><<<grid, kS3Threads, smem, s>>>(a, g.hnd ? nullptr : ctx->d_tmaps);
     return launched(ctx);
   }
   const size_t smem = static_cast<size_t>(g.C / kCluster) * g.token_bytes;
   if (smem > 200 * 1024) return B200KV_ENOTSUP;
   const uint32_t grid = kCluster * t.n_chunks() * g.planes;
   if (grid == 0) return B200KV_OK;
-  kv_fp8_store_kernel<<<grid, kFp8Threads, smem, s>>>(a);
+  kv_fp8_store_kernel<DT><<<grid, kFp8Threads, smem, s>>>(a);
   return launched(ctx);
 }
 
 // FP8 load, Q4 store and Q4 load of runs [f0, f0 + nf): one unit per (run, plane).
+template <int DT>
 int launch_per_run(b200kv_ctx* ctx, CopyMode mode, const TableView& tv, size_t f0, size_t nf, cudaStream_t s,
                    uint32_t plane_begin, uint32_t n_planes) {
   const bool fp8 = ctx->cfg.format == B200KV_FMT_FP8;
@@ -509,13 +514,14 @@ int launch_per_run(b200kv_ctx* ctx, CopyMode mode, const TableView& tv, size_t f
   a.total_units = static_cast<uint32_t>(nf) * a.n_planes;
   const uint32_t grid = std::min<uint32_t>(a.total_units, static_cast<uint32_t>(ctx->sm_count) * 8u);
   if (grid == 0) return B200KV_OK;
-  if (fp8) kv_fp8_load_kernel<<<grid, kFp8Threads, smem, s>>>(a);
-  else if (mode == kStore) kv_q4_store_kernel<<<grid, 256, 0, s>>>(a);
-  else kv_q4_load_kernel<<<grid, 256, 0, s>>>(a);
+  if (fp8) kv_fp8_load_kernel<DT><<<grid, kFp8Threads, smem, s>>>(a);
+  else if (mode == kStore) kv_q4_store_kernel<DT><<<grid, 256, 0, s>>>(a);
+  else kv_q4_load_kernel<DT><<<grid, 256, 0, s>>>(a);
   return launched(ctx);
 }
 
 // FP8 latent records of an MLA engine, either direction, runs [f0, f0 + nf): one warp per (run, plane) unit.
+template <int DT>
 int launch_mla_fp8(b200kv_ctx* ctx, CopyMode mode, const TableView& tv, size_t f0, size_t nf, cudaStream_t s,
                    uint32_t plane_begin, uint32_t n_planes) {
   KernelArgs a = kernel_args(ctx, tv, f0, plane_begin, n_planes);
@@ -523,9 +529,18 @@ int launch_mla_fp8(b200kv_ctx* ctx, CopyMode mode, const TableView& tv, size_t f
   constexpr uint32_t warps = kMlaThreads / 32;
   const uint32_t grid = std::min<uint32_t>((a.total_units + warps - 1) / warps, static_cast<uint32_t>(ctx->sm_count) * 8u);
   if (grid == 0) return B200KV_OK;
-  if (mode == kStore) kv_mla_fp8_store_kernel<<<grid, kMlaThreads, 0, s>>>(a);
-  else kv_mla_fp8_load_kernel<<<grid, kMlaThreads, 0, s>>>(a);
+  if (mode == kStore) kv_mla_fp8_store_kernel<DT><<<grid, kMlaThreads, 0, s>>>(a);
+  else kv_mla_fp8_load_kernel<DT><<<grid, kMlaThreads, 0, s>>>(a);
   return launched(ctx);
+}
+
+// The lossy launches of one cache element type.
+template <int DT>
+int launch_lossy(b200kv_ctx* ctx, CopyMode mode, const OpTable& t, const TableView& tv, size_t f0, size_t nf,
+                 cudaStream_t s, uint32_t pb, uint32_t np) {
+  if (ctx->cfg.format == B200KV_FMT_FP8 && ctx->g.mla) return launch_mla_fp8<DT>(ctx, mode, tv, f0, nf, s, pb, np);
+  if (ctx->cfg.format == B200KV_FMT_FP8 && mode == kStore) return launch_fp8_store<DT>(ctx, t, tv, s);
+  return launch_per_run<DT>(ctx, mode, tv, f0, nf, s, pb, np);
 }
 
 // Launches the kernels that move chunks [c0, c1) of table t, planes [pb, pb + np) (np == 0: every plane), in
@@ -535,9 +550,9 @@ int launch_op(b200kv_ctx* ctx, CopyMode mode, const OpTable& t, const TableView&
               cudaStream_t s, uint32_t pb = 0, uint32_t np = 0, const Peer* peer = nullptr) {
   const size_t f0 = t.full_off[c0], nf = t.full_off[c1] - f0;
   const int fmt = mode == kPull ? B200KV_FMT_RAW : ctx->cfg.format;
-  if (fmt == B200KV_FMT_FP8 && ctx->g.mla) return launch_mla_fp8(ctx, mode, tv, f0, nf, s, pb, np);
-  if (fmt == B200KV_FMT_FP8 && mode == kStore) return launch_fp8_store(ctx, t, tv, s);
-  if (fmt != B200KV_FMT_RAW) return launch_per_run(ctx, mode, tv, f0, nf, s, pb, np);
+  if (fmt != B200KV_FMT_RAW)
+    return ctx->g.dtype == B200KV_DTYPE_FP16 ? launch_lossy<kFp16>(ctx, mode, t, tv, f0, nf, s, pb, np)
+                                             : launch_lossy<kBf16>(ctx, mode, t, tv, f0, nf, s, pb, np);
   const size_t p0 = t.n_full() + t.part_off[c0], n_part = t.part_off[c1] - t.part_off[c0];
   switch (mode) {
     case kStore: return launch_copy_runs<kStore>(ctx, tv, f0, nf, p0, n_part, s, peer, pb, np);
@@ -805,10 +820,13 @@ static int engine_create_impl(const b200kv_engine_config* cfg, b200kv_pool* pool
                          bulk_kernel<kPull>(ctx->S, ctx->LAG)})
       if (k) CU_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   }
-  if (cfg->format == B200KV_FMT_FP8 && !g.mla) {
-    CU_TRY(cudaFuncSetAttribute(kv_fp8_store3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  if (cfg->format == B200KV_FMT_FP8 && !g.mla) {   // both element types: b200kv_set_cache_dtype comes later
+    CU_TRY(cudaFuncSetAttribute(kv_fp8_store3_kernel<kBf16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 kS3Stages * kS3MaxUnitBytes));
-    CU_TRY(cudaFuncSetAttribute(kv_fp8_store_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    CU_TRY(cudaFuncSetAttribute(kv_fp8_store_kernel<kBf16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    CU_TRY(cudaFuncSetAttribute(kv_fp8_store3_kernel<kFp16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                kS3Stages * kS3MaxUnitBytes));
+    CU_TRY(cudaFuncSetAttribute(kv_fp8_store_kernel<kFp16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   }
 
   CU_TRY(cudaMalloc(&ctx->d_bases, sizeof(uint64_t) * g.planes));
@@ -949,6 +967,15 @@ static void build_tensor_maps(b200kv_ctx* ctx, const std::vector<uint64_t>& base
     return;
   }
   ctx->tmap_status = "ok";
+}
+
+extern "C" int b200kv_set_cache_dtype(b200kv_ctx* ctx, int32_t dtype) {
+  if (!ctx || (dtype != B200KV_DTYPE_BF16 && dtype != B200KV_DTYPE_FP16)) return B200KV_EINVAL;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  if (ctx->kv_registered) return B200KV_EBUSY;   // chunks already stored or moved under the old type
+  if (dtype == B200KV_DTYPE_FP16 && ctx->g.elem != 2) return B200KV_EINVAL;
+  ctx->g.dtype = static_cast<uint32_t>(dtype);
+  return B200KV_OK;
 }
 
 extern "C" int b200kv_register_kv(b200kv_ctx* ctx, const void* const* k_ptrs,

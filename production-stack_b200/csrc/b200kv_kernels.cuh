@@ -32,7 +32,8 @@
 //   kv_mla_fp8_store_kernel /  FP8 latent records of MLA engines: one warp per (token, plane), a group of
 //   kv_mla_fp8_load_kernel     128 elements is 16 lanes; no shared memory.
 //
-// Every kernel takes one KernelArgs, filled by kernel_args() in b200kv_engine.cu.
+// Every kernel takes one KernelArgs, filled by kernel_args() in b200kv_engine.cu.  The seven FP8 / Q4 / MLA FP8
+// kernels are also built per cache element type (bf16, fp16: template argument DT, see Src below).
 #pragma once
 
 #include <cuda_bf16.h>
@@ -75,7 +76,7 @@ struct KernelArgs {
   uint32_t pieces;                // bulk copy: pieces per run = ceil(block_tokens / piece_tokens)
   uint32_t piece_tokens;          // bulk copy: tokens per piece (piece bytes <= stage bytes)
   uint32_t total_units;           // units of work of the launch; each kernel says what its unit is
-  uint32_t row_bytes;             // D * elem: one (token, head) row (D*2 for FP8 / Q4, which take bf16 only)
+  uint32_t row_bytes;             // D * elem: one (token, head) row (D*2 for FP8 / Q4, which take 16-bit caches only)
   uint32_t hnd;                   // pages hold [H][block_tokens][D] tiles
 };
 static_assert(sizeof(KernelArgs) <= 128, "KernelArgs must stay within 128 bytes (see above)");
@@ -380,20 +381,64 @@ constexpr int kCluster = 8;
 constexpr int kFp8Threads = 256;
 constexpr int kMaxHeads = 64;
 
+// |x| max of packed 16-bit pairs: the sign bit cleared, integer order equals magnitude order for bf16 and fp16 alike
 __device__ __forceinline__ uint32_t absmax_u16x2(uint32_t acc, uint32_t w) {
   return __vmaxu2(acc, w & 0x7fff7fffu);
 }
 
-// e4m3 of 8 bf16 scaled by inv (fp32 multiply, RN, satfinite) -> 8 bytes.
+// ---------------------------------------------------------------------------------------------
+// Element type of the paged cache the lossy kernels read and write (B200KV_DTYPE_*).  It is a template argument,
+// not a KernelArgs field (see the 128-byte note on KernelArgs).  Everything else about a format is the same for
+// both types: the absmax is taken on the 16-bit magnitude bits, quantisation works on the exact fp32 value, and
+// decoding rounds the fp32 product once to the cache's type (RN).  Q4 scales stay bf16 bits in either case.
+// Specification of the fp16 builds: tests/fp16_oracle.py.
+// ---------------------------------------------------------------------------------------------
+enum CacheDtype { kBf16 = 0, kFp16 = 1 };
+
+template <int DT>
+struct Src;
+template <>
+struct Src<kBf16> {
+  // the two elements of a packed pair as fp32: lo = element 0 (low half), hi = element 1
+  static __device__ __forceinline__ float lo(uint32_t w) { return __uint_as_float(w << 16); }
+  static __device__ __forceinline__ float hi(uint32_t w) { return __uint_as_float(w & 0xffff0000u); }
+  // two fp32 -> a packed pair, round to nearest even
+  static __device__ __forceinline__ uint32_t pack_rn(float a, float b) {
+    const __nv_bfloat162 r = __floats2bfloat162_rn(a, b);
+    return *reinterpret_cast<const uint32_t*>(&r);
+  }
+  // 16-bit magnitude bits (an absmax) -> fp32
+  static __device__ __forceinline__ float from_bits(uint32_t m) { return __uint_as_float(m << 16); }
+};
+template <>
+struct Src<kFp16> {
+  // two scalar conversions: __half22float2 costs kv_q4_store_kernel 4 registers (39 -> 43) and so one CTA per SM
+  static __device__ __forceinline__ float lo(uint32_t w) {
+    return __half2float(__ushort_as_half(static_cast<unsigned short>(w & 0xffffu)));
+  }
+  static __device__ __forceinline__ float hi(uint32_t w) {
+    return __half2float(__ushort_as_half(static_cast<unsigned short>(w >> 16)));
+  }
+  static __device__ __forceinline__ uint32_t pack_rn(float a, float b) {
+    const __half2 r = __floats2half2_rn(a, b);
+    return *reinterpret_cast<const uint32_t*>(&r);
+  }
+  static __device__ __forceinline__ float from_bits(uint32_t m) {
+    return __half2float(__ushort_as_half(static_cast<unsigned short>(m)));
+  }
+};
+
+// e4m3 of 8 cache elements scaled by inv (fp32 multiply, RN, satfinite) -> 8 bytes.
+template <int DT>
 __device__ __forceinline__ uint2 quant8(const uint4& v, float inv) {
   const uint32_t w[4] = {v.x, v.y, v.z, v.w};
   uint32_t o[2];
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
-    const float a0 = __uint_as_float(w[2 * i] << 16) * inv;
-    const float a1 = __uint_as_float(w[2 * i] & 0xffff0000u) * inv;
-    const float b0 = __uint_as_float(w[2 * i + 1] << 16) * inv;
-    const float b1 = __uint_as_float(w[2 * i + 1] & 0xffff0000u) * inv;
+    const float a0 = Src<DT>::lo(w[2 * i]) * inv;
+    const float a1 = Src<DT>::hi(w[2 * i]) * inv;
+    const float b0 = Src<DT>::lo(w[2 * i + 1]) * inv;
+    const float b1 = Src<DT>::hi(w[2 * i + 1]) * inv;
     const uint32_t lo = __nv_cvt_float2_to_fp8x2(make_float2(a0, a1), __NV_SATFINITE, __NV_E4M3);
     const uint32_t hi = __nv_cvt_float2_to_fp8x2(make_float2(b0, b1), __NV_SATFINITE, __NV_E4M3);
     o[i] = lo | (hi << 16);
@@ -401,11 +446,12 @@ __device__ __forceinline__ uint2 quant8(const uint4& v, float inv) {
   return make_uint2(o[0], o[1]);
 }
 
+template <int DT>
 __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kFp8Threads)
     kv_fp8_store_kernel(const KernelArgs p) {
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ __align__(8) uint64_t bar;
-  __shared__ uint32_t s_absmax[kMaxHeads];  // this CTA's |x| max per head (bf16 bits: integer order == magnitude)
+  __shared__ uint32_t s_absmax[kMaxHeads];  // this CTA's |x| max per head (16-bit magnitude bits)
   __shared__ uint32_t s_all[kMaxHeads];     // cluster-wide max: every CTA pushes its value into every CTA's copy
   __shared__ float s_inv[kMaxHeads];
 
@@ -533,7 +579,7 @@ __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kFp8Threads)
 
   if (threadIdx.x < p.n_heads) {
     const uint32_t m = s_all[threadIdx.x];
-    const float amax = __uint_as_float(m << 16);
+    const float amax = Src<DT>::from_bits(m);
     const float inv = (m == 0) ? 1.0f : __fdiv_rn(448.0f, amax);
     s_inv[threadIdx.x] = inv;
     if (rank == 0) {
@@ -557,7 +603,7 @@ __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kFp8Threads)
 #pragma unroll 8
         for (uint32_t v = lane; v < nv; v += 32) {
           const uint4 x = *reinterpret_cast<const uint4*>(smem + (base + v) * 16);
-          st_na_v2(outh + (base + v) * 8, quant8(x, inv));
+          st_na_v2(outh + (base + v) * 8, quant8<DT>(x, inv));
         }
       }
     }
@@ -573,13 +619,13 @@ __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kFp8Threads)
     const float inv = s_inv[((threadIdx.x % vpt) * 16) / p.row_bytes];
     for (uint32_t i = threadIdx.x; i < nvec; i += kFp8Threads) {
       const uint4 v = *reinterpret_cast<const uint4*>(smem + static_cast<size_t>(i) * 16);
-      st_na_v2(out + static_cast<size_t>(i) * 8, quant8(v, inv));
+      st_na_v2(out + static_cast<size_t>(i) * 8, quant8<DT>(v, inv));
     }
   } else {
     for (uint32_t i = threadIdx.x; i < nvec; i += kFp8Threads) {
       const uint32_t col = i % vpt;
       const uint4 v = *reinterpret_cast<const uint4*>(smem + static_cast<size_t>(i) * 16);
-      st_na_v2(out + static_cast<size_t>(i) * 8, quant8(v, s_inv[(col * 16) / p.row_bytes]));
+      st_na_v2(out + static_cast<size_t>(i) * 8, quant8<DT>(v, s_inv[(col * 16) / p.row_bytes]));
     }
   }
 }
@@ -634,6 +680,7 @@ __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t n_threads) 
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n_threads) : "memory");
 }
 
+template <int DT>
 __global__ void __launch_bounds__(kS3Threads, 1) kv_fp8_store3_kernel(const KernelArgs p,
                      const void* tmaps) {   // one CUtensorMap per plane (NHD pages); nullptr for HND pages
   extern __shared__ __align__(128) uint8_t smem[];
@@ -732,7 +779,7 @@ __global__ void __launch_bounds__(kS3Threads, 1) kv_fp8_store3_kernel(const Kern
     uint32_t m = 0;
 #pragma unroll
     for (int w = 0; w < kS3GroupThreads / 32; ++w) m = max(m, s_max[g][par][w]);
-    const float amax = __uint_as_float(m << 16);
+    const float amax = Src<DT>::from_bits(m);
     const float inv = (m == 0) ? 1.0f : __fdiv_rn(448.0f, amax);
     const uint64_t chunk_base = __ldg(p.chunk.chunk_addrs + c);
     if (t == 0) {
@@ -754,15 +801,16 @@ __global__ void __launch_bounds__(kS3Threads, 1) kv_fp8_store3_kernel(const Kern
     uint8_t* dst = slab + off0;
 #pragma unroll
     for (int kk = 0; kk < kS3MaxVec; ++kk) {
-      if (tok0 + kk * tok_step < n_valid) st_na_v2(dst + static_cast<size_t>(kk) * off_step, quant8(x[kk], inv));
+      if (tok0 + kk * tok_step < n_valid) st_na_v2(dst + static_cast<size_t>(kk) * off_step, quant8<DT>(x[kk], inv));
     }
   }
 }
 
 // ---------------------------------------------------------------------------------------------
-// FP8 load: one CTA per (run, plane) unit (total_units = n_runs * n_planes); e4m3 * scale -> bf16 (RN)
-// into the pages.
+// FP8 load: one CTA per (run, plane) unit (total_units = n_runs * n_planes); e4m3 * scale -> the cache's type
+// (one RN rounding of the fp32 product) into the pages.
 // ---------------------------------------------------------------------------------------------
+template <int DT>
 __device__ __forceinline__ uint4 dequant8(const uint2& q, float scale) {
   const uint32_t w[2] = {q.x, q.y};
   uint32_t o[4];
@@ -772,19 +820,18 @@ __device__ __forceinline__ uint4 dequant8(const uint2& q, float scale) {
     const __half2_raw h1 = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(w[i] >> 16), __NV_E4M3);
     const float2 f0 = __half22float2(*reinterpret_cast<const __half2*>(&h0));
     const float2 f1 = __half22float2(*reinterpret_cast<const __half2*>(&h1));
-    const __nv_bfloat162 b0 = __floats2bfloat162_rn(f0.x * scale, f0.y * scale);
-    const __nv_bfloat162 b1 = __floats2bfloat162_rn(f1.x * scale, f1.y * scale);
-    o[2 * i] = *reinterpret_cast<const uint32_t*>(&b0);
-    o[2 * i + 1] = *reinterpret_cast<const uint32_t*>(&b1);
+    o[2 * i] = Src<DT>::pack_rn(f0.x * scale, f0.y * scale);
+    o[2 * i + 1] = Src<DT>::pack_rn(f1.x * scale, f1.y * scale);
   }
   return make_uint4(o[0], o[1], o[2], o[3]);
 }
 
+template <int DT>
 __global__ void __launch_bounds__(kFp8Threads) kv_fp8_load_kernel(const KernelArgs p) {
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ __align__(8) uint64_t bar;
   __shared__ float s_scale[kMaxHeads];
-  const uint32_t tb = p.paged.token_bytes;  // bf16 bytes per token
+  const uint32_t tb = p.paged.token_bytes;  // 16-bit cache bytes per token
   const uint32_t qtb = tb >> 1;
 
   if (threadIdx.x == 0) {
@@ -828,7 +875,7 @@ __global__ void __launch_bounds__(kFp8Threads) kv_fp8_load_kernel(const KernelAr
         const uint2 q = *reinterpret_cast<const uint2*>(smem + (static_cast<size_t>(h) * bs + o_src + r) * (p.row_bytes >> 1) +
                                                         static_cast<size_t>(cc) * 8);
         uint8_t* d = reinterpret_cast<uint8_t*>(paged_addr_hnd(p.paged, plane, static_cast<uint32_t>(run.a), h, p.row_bytes));
-        st_na_v4(d + static_cast<size_t>(r) * p.row_bytes + static_cast<size_t>(cc) * 16, dequant8(q, s_scale[h]));
+        st_na_v4(d + static_cast<size_t>(r) * p.row_bytes + static_cast<size_t>(cc) * 16, dequant8<DT>(q, s_scale[h]));
       }
       __syncthreads();
       continue;
@@ -839,13 +886,13 @@ __global__ void __launch_bounds__(kFp8Threads) kv_fp8_load_kernel(const KernelAr
       const float sc = s_scale[((threadIdx.x % vpt) * 16) / p.row_bytes];
       for (uint32_t i = threadIdx.x; i < nvec; i += kFp8Threads) {
         const uint2 q = *reinterpret_cast<const uint2*>(smem + static_cast<size_t>(i) * 8);
-        st_na_v4(dst + static_cast<size_t>(i) * 16, dequant8(q, sc));
+        st_na_v4(dst + static_cast<size_t>(i) * 16, dequant8<DT>(q, sc));
       }
     } else {
       for (uint32_t i = threadIdx.x; i < nvec; i += kFp8Threads) {
         const uint32_t col = i % vpt;
         const uint2 q = *reinterpret_cast<const uint2*>(smem + static_cast<size_t>(i) * 8);
-        st_na_v4(dst + static_cast<size_t>(i) * 16, dequant8(q, s_scale[(col * 16) / p.row_bytes]));
+        st_na_v4(dst + static_cast<size_t>(i) * 16, dequant8<DT>(q, s_scale[(col * 16) / p.row_bytes]));
       }
     }
     __syncthreads();  // smem + s_scale reusable
@@ -877,7 +924,9 @@ __device__ __forceinline__ void q4_split(uint32_t idx, uint32_t vpt, uint32_t vp
 }
 
 // q = rint(x * inv) (exact product, ties to even), inv = fl32(1 / s), s = bf16(absmax_group / 7)
-// (oracle/kv_oracle.py q4_pack_chunk): one IEEE division per group, then one FMA per element.
+// (oracle/kv_oracle.py q4_pack_chunk): one IEEE division per group, then one FMA per element.  The scale is bf16
+// for fp16 caches too.
+template <int DT>
 __global__ void __launch_bounds__(256) kv_q4_store_kernel(const KernelArgs p) {
   const uint32_t vpt = (p.n_heads * p.row_bytes) >> 4;      // vectors per token (multiple of 4)
   const uint32_t vpt_shift = (vpt & (vpt - 1)) == 0 ? 31u - __clz(vpt) : 0xffffffffu;
@@ -909,7 +958,7 @@ __global__ void __launch_bounds__(256) kv_q4_store_kernel(const KernelArgs p) {
         uint32_t m = max(acc & 0xffffu, acc >> 16);
         m = max(m, __shfl_xor_sync(0xffffffffu, m, 1));
         m = max(m, __shfl_xor_sync(0xffffffffu, m, 2));
-        const float amax = __uint_as_float(m << 16);
+        const float amax = Src<DT>::from_bits(m);
         const __nv_bfloat16 sb = m ? __float2bfloat16_rn(__fdiv_rn(amax, 7.0f)) : __float2bfloat16_rn(1.0f);
         const float inv = __fdiv_rn(1.0f, __bfloat162float(sb));
         // rint(x * inv) for |x * inv| <= 7.03 without a convert: fma(x, inv, 1.5 * 2^23) rounds the EXACT product to
@@ -919,7 +968,7 @@ __global__ void __launch_bounds__(256) kv_q4_store_kernel(const KernelArgs p) {
         uint32_t packed = 0;
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-          const float lo = __uint_as_float(w[i] << 16), hi = __uint_as_float(w[i] & 0xffff0000u);
+          const float lo = Src<DT>::lo(w[i]), hi = Src<DT>::hi(w[i]);
           const uint32_t ql = __float_as_uint(__fmaf_rn(lo, inv, 12582912.0f)) & 0xFu;
           const uint32_t qh = __float_as_uint(__fmaf_rn(hi, inv, 12582912.0f)) & 0xFu;
           packed |= (ql | (qh << 4)) << (8 * i);
@@ -933,6 +982,7 @@ __global__ void __launch_bounds__(256) kv_q4_store_kernel(const KernelArgs p) {
   }
 }
 
+template <int DT>
 __global__ void __launch_bounds__(256) kv_q4_load_kernel(const KernelArgs p) {
   const uint32_t vpt = (p.n_heads * p.row_bytes) >> 4;
   const uint32_t vpt_shift = (vpt & (vpt - 1)) == 0 ? 31u - __clz(vpt) : 0xffffffffu;
@@ -970,8 +1020,7 @@ __global__ void __launch_bounds__(256) kv_q4_load_kernel(const KernelArgs p) {
         for (int i = 0; i < 4; ++i) {
           const int b = static_cast<int>((packed[j] >> (8 * i)) & 0xffu);
           const int ql = ((b & 0xF) ^ 8) - 8, qh = ((b >> 4) ^ 8) - 8;   // sign-extend the nibbles
-          const __nv_bfloat162 r = __floats2bfloat162_rn(static_cast<float>(ql) * s, static_cast<float>(qh) * s);
-          o[i] = *reinterpret_cast<const uint32_t*>(&r);
+          o[i] = Src<DT>::pack_rn(static_cast<float>(ql) * s, static_cast<float>(qh) * s);
         }
         st_na_v4(reinterpret_cast<void*>(q4_src_addr(p, plane, static_cast<uint32_t>(run.a) + tt[j], vv[j])),
                  make_uint4(o[0], o[1], o[2], o[3]));
@@ -981,9 +1030,11 @@ __global__ void __launch_bounds__(256) kv_q4_load_kernel(const KernelArgs p) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// FP8 latent records of an MLA engine (B200KV_LAYOUT_MLA + B200KV_FMT_FP8; spec: tests/mla_oracle.py).
-// A bf16 page row is 576 elements = 72 16-byte vectors: latent vectors 0..63 (group g = vectors
-// [16g, 16g+16)), RoPE vectors 64..71.  A record is [512 e4m3 codes][4 fp32 scales][64 bf16 RoPE].
+// FP8 latent records of an MLA engine (B200KV_LAYOUT_MLA + B200KV_FMT_FP8; spec: tests/mla_oracle.py, and
+// tests/fp16_oracle.py for fp16 caches).
+// A page row is 576 16-bit elements = 72 16-byte vectors: latent vectors 0..63 (group g = vectors
+// [16g, 16g+16)), RoPE vectors 64..71.  A record is [512 e4m3 codes][4 fp32 scales][64 RoPE elements in the
+// cache's own type].
 // One warp per (token, plane): lane l holds latent vectors l and l+32, so lanes 0-15 see groups 0 and 2 and
 // lanes 16-31 groups 1 and 3, and each half reduces both of its groups at once with four shuffles of two
 // packed bf16 magnitudes.  Lane l writes 8 code bytes per vector (256 contiguous bytes per warp and vector),
@@ -998,15 +1049,18 @@ constexpr uint32_t kMlaRopeOff = 528;        // 33 * 16
 constexpr int kMlaThreads = 256;
 constexpr int kMlaTokens = 4;
 
-// scale = fl32(absmax / 448), inv = fl32(448 / absmax), both 1 when absmax is 0 (m = bf16 bits of absmax)
-__device__ __forceinline__ float mla_scale(uint32_t m) { return m ? __fdiv_rn(__uint_as_float(m << 16), 448.0f) : 1.0f; }
-__device__ __forceinline__ float mla_inv(uint32_t m) { return m ? __fdiv_rn(448.0f, __uint_as_float(m << 16)) : 1.0f; }
+// scale = fl32(absmax / 448), inv = fl32(448 / absmax), both 1 when absmax is 0 (m = 16-bit magnitude bits of absmax)
+template <int DT>
+__device__ __forceinline__ float mla_scale(uint32_t m) { return m ? __fdiv_rn(Src<DT>::from_bits(m), 448.0f) : 1.0f; }
+template <int DT>
+__device__ __forceinline__ float mla_inv(uint32_t m) { return m ? __fdiv_rn(448.0f, Src<DT>::from_bits(m)) : 1.0f; }
 
 __device__ __forceinline__ uint32_t absmax_vec(const uint4& v) {
   const uint32_t acc = absmax_u16x2(absmax_u16x2(absmax_u16x2(absmax_u16x2(0u, v.x), v.y), v.z), v.w);
   return max(acc & 0xffffu, acc >> 16);
 }
 
+template <int DT>
 __global__ void __launch_bounds__(kMlaThreads) kv_mla_fp8_store_kernel(const KernelArgs p) {
   const uint32_t lane = threadIdx.x & 31u;
   const uint32_t n_warps = gridDim.x * (kMlaThreads / 32);
@@ -1034,11 +1088,11 @@ __global__ void __launch_bounds__(kMlaThreads) kv_mla_fp8_store_kernel(const Ker
         m = __vmaxu2(m, __shfl_xor_sync(0xffffffffu, m, 8));
         const uint32_t other = __shfl_xor_sync(0xffffffffu, m, 16);
         uint8_t* rec = reinterpret_cast<uint8_t*>(chunk_addr(p.chunk, plane, static_cast<uint32_t>(run.b + j + k)));
-        st_na_v2(rec + 8 * lane, quant8(a[k], mla_inv(m & 0xffffu)));
-        st_na_v2(rec + 256 + 8 * lane, quant8(b[k], mla_inv(m >> 16)));
+        st_na_v2(rec + 8 * lane, quant8<DT>(a[k], mla_inv<DT>(m & 0xffffu)));
+        st_na_v2(rec + 256 + 8 * lane, quant8<DT>(b[k], mla_inv<DT>(m >> 16)));
         if (lane == 0) {
-          const float4 s = make_float4(mla_scale(m & 0xffffu), mla_scale(other & 0xffffu), mla_scale(m >> 16),
-                                       mla_scale(other >> 16));
+          const float4 s = make_float4(mla_scale<DT>(m & 0xffffu), mla_scale<DT>(other & 0xffffu), mla_scale<DT>(m >> 16),
+                                       mla_scale<DT>(other >> 16));
           st_na_v4(rec + kMlaScalesOff, *reinterpret_cast<const uint4*>(&s));
         }
         if (lane < 8) st_na_v4(rec + kMlaRopeOff + 16 * lane, r[k]);
@@ -1047,6 +1101,7 @@ __global__ void __launch_bounds__(kMlaThreads) kv_mla_fp8_store_kernel(const Ker
   }
 }
 
+template <int DT>
 __global__ void __launch_bounds__(kMlaThreads) kv_mla_fp8_load_kernel(const KernelArgs p) {
   const uint32_t lane = threadIdx.x & 31u;
   const uint32_t half = lane >> 4;
@@ -1075,8 +1130,8 @@ __global__ void __launch_bounds__(kMlaThreads) kv_mla_fp8_load_kernel(const Kern
       for (int k = 0; k < kMlaTokens; ++k) {
         if (j + k >= run.n) break;
         uint8_t* row = reinterpret_cast<uint8_t*>(paged_addr(p.paged, plane, static_cast<uint32_t>(run.a + j + k)));
-        st_na_v4(row + 16 * lane, dequant8(qa[k], sa[k]));
-        st_na_v4(row + 512 + 16 * lane, dequant8(qb[k], sb[k]));
+        st_na_v4(row + 16 * lane, dequant8<DT>(qa[k], sa[k]));
+        st_na_v4(row + 512 + 16 * lane, dequant8<DT>(qb[k], sb[k]));
         if (lane < 8) st_na_v4(row + 1024 + 16 * lane, r[k]);
       }
     }
