@@ -94,6 +94,13 @@ extern "C" {
  *      or fp16 cache and D == 576; Q4 is not offered on MLA (-ENOTSUP).  In an fp16 cache the RoPE part
  *      is fp16 bits, where vLLM's fp8_ds_mla has bf16; such chunks carry the fp16 format tag.      */
 #define B200KV_LAYOUT_MLA 2
+/* Indexer planes (MLA with DeepSeek Sparse Attention: DeepSeek-V3.2).  After b200kv_set_indexer an MLA engine also
+ *      moves one indexer plane per layer, verbatim, on every path.  vLLM's indexer_k_quant_and_cache writes a block
+ *      of such a plane as a split tile: [block_tokens][value_bytes] e4m3 values, then [block_tokens][scale_bytes]
+ *      (one fp32 scale per token); V3.2 has 128 + 4.  A chunk is the MLA chunk above (RAW slabs or FP8 records,
+ *      not rounded) followed by L indexer slabs, each [C][value_bytes] then [C][scale_bytes], and the whole is
+ *      rounded up to 256 bytes.  Such chunks carry bit 24 in their format tag (format | layout << 8 |
+ *      dtype << 16 | 1 << 24).                                                                   */
 
 /* ---- kernel variants (both are CUDA; selectable for A/B measurement) ------------------- */
 #define B200KV_VARIANT_BULK 0 /* cp.async.bulk (TMA engine) through a shared-memory ring    */
@@ -250,18 +257,32 @@ int b200kv_engine_create(const b200kv_engine_config* cfg, b200kv_pool* pool, b20
  * b200kv_register_kv: -EBUSY after registration.  FP16 needs elem_bytes == 2, else -EINVAL.  A function
  * rather than a config field, so the v1 config layout and every existing binding stay valid.     */
 int b200kv_set_cache_dtype(b200kv_ctx* ctx, int32_t dtype);
+/* Gives an MLA engine an indexer plane per layer (B200KV_LAYOUT_MLA, indexer planes above); block_stride_bytes is
+ * the bytes between consecutive blocks of one indexer plane (>= block_tokens * (value_bytes + scale_bytes), a
+ * multiple of 16).  value_bytes % 16 == 0, scale_bytes % 4 == 0.  Legal between b200kv_engine_create and
+ * b200kv_register_kv (and before b200kv_tier_create): -EBUSY after; -EINVAL on an engine that is not MLA.  The
+ * staging ring is re-cut to the larger chunk; a pool whose slots are smaller than it gives -EINVAL.  From then on
+ * b200kv_register_kv and b200kv_import_peer_ptrs take the indexer planes in v_ptrs, b200kv_export_ipc /
+ * b200kv_import_peer take 2*L descriptors (latent planes, then indexer planes), and a peer's indexer planes are
+ * taken to have this engine's indexer block stride.                                           */
+int b200kv_set_indexer(b200kv_ctx* ctx, int32_t value_bytes, int32_t scale_bytes, uint64_t block_stride_bytes);
 /* What the engine did about host-page placement when it pinned the pool (numa_policy above), as text
  * for logs and bench output, e.g. "mbind preferred node 1".                                  */
 int b200kv_engine_numa_placement(b200kv_ctx* ctx, char* buf, uint64_t n);
 int b200kv_engine_destroy(b200kv_ctx* ctx);
 /* chunk_bytes for this engine's format — slot_bytes a pool must be created with.           */
 int64_t b200kv_engine_chunk_bytes(const b200kv_engine_config* cfg);
+/* chunk_bytes of the same engine after b200kv_set_indexer(ctx, value_bytes, scale_bytes, ...):
+ * round_up(latent + L * C * (value_bytes + scale_bytes), 256), latent = L * C * D * elem_bytes (RAW) or
+ * L * C * 656 (FP8 records).  -EINVAL for a geometry that is not MLA.                         */
+int64_t b200kv_engine_chunk_bytes_indexed(const b200kv_engine_config* cfg, int32_t value_bytes, int32_t scale_bytes);
 
 /* register_kv_caches (KVConnectorBase_V1, vllm/.../v1/base.py:251): device base address of
  * block 0 of each layer's K and V planes, NHD within a block ([block_tokens][H][D]).
  * FlashAttention (2,NB,bs,H,D): v = k + NB*tile; FlashInfer (NB,2,bs,H,D): v = k + tile,
  * block_stride = 2*tile; cross-layer (NB,L,2,bs,H,D): block_stride = 2*L*tile.
- * B200KV_LAYOUT_MLA: k_ptrs are the layers' latent planes and v_ptrs must be NULL.           */
+ * B200KV_LAYOUT_MLA: k_ptrs are the layers' latent planes and v_ptrs must be NULL, or the layers' indexer
+ * planes after b200kv_set_indexer.                                                           */
 int b200kv_register_kv(b200kv_ctx* ctx, const void* const* k_ptrs, const void* const* v_ptrs);
 
 /* lmcache_engine.store (vllm_v1_adapter.py:1115-1123).  Tokens [0,n_tokens) start on a
@@ -339,8 +360,9 @@ typedef struct b200kv_ipc_desc {
 } b200kv_ipc_desc;
 
 /* Export 2*L descriptors (K planes then V planes) of the registered cache; L (one per layer's
- * latent plane) for B200KV_LAYOUT_MLA.  import_peer takes as many; import_peer_ptrs takes
- * v_ptrs NULL for MLA.                                                                     */
+ * latent plane) for B200KV_LAYOUT_MLA, 2*L (latent planes then indexer planes) after
+ * b200kv_set_indexer.  import_peer takes as many; import_peer_ptrs takes v_ptrs NULL for MLA,
+ * and the indexer planes in v_ptrs after b200kv_set_indexer.                               */
 int b200kv_export_ipc(b200kv_ctx* ctx, b200kv_ipc_desc* descs_out, int32_t n_descs);
 /* Map a peer replica's cache (same model geometry).  `peer_id` is caller-chosen (0..63).   */
 int b200kv_import_peer(b200kv_ctx* ctx, int32_t peer_id, int32_t peer_device,

@@ -16,6 +16,7 @@ FMT_RAW, FMT_FP8, FMT_Q4 = 0, 1, 2   # FMT_Q4: experimental (group-wise 4-bit)
 VARIANT_BULK, VARIANT_LDG = 0, 1
 LAYOUT_NHD, LAYOUT_HND, LAYOUT_MLA = 0, 1, 2   # LAYOUT_MLA: one latent plane per layer (DeepSeek-V2/V3, Kimi-K2)
 DTYPE_BF16, DTYPE_FP16 = 0, 1                  # element type of the cache (b200kv_set_cache_dtype)
+FMT_TAG_INDEXED = 1 << 24                      # format-tag bit of chunks with indexer planes (b200kv_set_indexer)
 POOL_CREATE, POOL_ATTACH, POOL_CREATE_OR_ATTACH = 1, 2, 3
 NUMA_LOCAL, NUMA_INTERLEAVE, NUMA_OFF = 0, 1, 2
 
@@ -93,8 +94,10 @@ SIGNATURES = {
     "b200kv_engine_create": (C.c_int, [C.POINTER(EngineConfig), _P, C.POINTER(_P)]),
     "b200kv_engine_destroy": (C.c_int, [_P]),
     "b200kv_set_cache_dtype": (C.c_int, [_P, C.c_int32]),
+    "b200kv_set_indexer": (C.c_int, [_P, C.c_int32, C.c_int32, C.c_uint64]),
     "b200kv_engine_numa_placement": (C.c_int, [_P, C.c_char_p, C.c_uint64]),
     "b200kv_engine_chunk_bytes": (C.c_int64, [C.POINTER(EngineConfig)]),
+    "b200kv_engine_chunk_bytes_indexed": (C.c_int64, [C.POINTER(EngineConfig), C.c_int32, C.c_int32]),
     "b200kv_register_kv": (C.c_int, [_P, C.POINTER(_P), C.POINTER(_P)]),
     "b200kv_store_async": (C.c_int, [_P, _U64P, C.c_int32, _I64P, C.c_int64, _P, _U64P]),
     "b200kv_load_async": (C.c_int, [_P, _U64P, C.c_int32, _I64P, C.c_int64, C.c_int32, _P, _U64P, _I64P]),

@@ -25,7 +25,8 @@ from vllm.distributed.kv_transfer.kv_connector.v1.base import (KVConnectorBase_V
 from . import _lib
 from .adapter import ReqMeta, SchedulerState, WorkerState, request_identity
 from .config import B200KVConfig
-from .engine import KVEngine, KVGeometry, KVPool, dtype_code, paged_layout_of, xxh64
+from .engine import (INDEXER_SCALE_BYTES, INDEXER_VALUE_BYTES, KVEngine, KVGeometry, KVPool, dtype_code,
+                     paged_layout_of, split_indexer_caches, xxh64)
 from .pd import PDMeta, PDScheduler, PDWorker, first_group, publish_ipc, unpublish_ipc
 
 if TYPE_CHECKING:
@@ -74,7 +75,10 @@ def geometry_from_vllm(vllm_config, cfg: B200KVConfig, n_blocks: int = 1) -> KVG
     (vllm_v1_adapter.py:471-477), derivable in both roles from the vLLM config alone.  An MLA model
     (model_config.use_mla) has one latent plane per layer: (num_layer, 1, chunk, 1, head_size)
     (vllm_v1_adapter.py:463-477).  The cache's element type: the model's with cache_dtype "auto",
-    named by "float16" / "bfloat16"; every other cache dtype (fp8*, ...) keeps bf16, which only RAW reads."""
+    named by "float16" / "bfloat16"; every other cache dtype (fp8*, ...) keeps bf16, which only RAW reads.
+    An MLA model with DeepSeek Sparse Attention (DeepSeek-V3.2: index_topk in the HF config, vLLM's test) also
+    has an indexer key cache per layer, which the geometry's indexer planes describe.  With the fp8_ds_mla cache a
+    latent token is already a 656-byte FP8 record, so the chunk stores it RAW, also when FP8 is asked for."""
     mc, pc, cc = vllm_config.model_config, vllm_config.parallel_config, vllm_config.cache_config
     dt = str(cc.cache_dtype)
     dtype = _lib.DTYPE_BF16
@@ -87,10 +91,30 @@ def geometry_from_vllm(vllm_config, cfg: B200KVConfig, n_blocks: int = 1) -> KVG
         if dt == "float16":
             dtype = _lib.DTYPE_FP16
     mla = bool(getattr(mc, "use_mla", False))
+    head_dim, fmt = mc.get_head_size(), cfg.fmt
+    if mla and dt == "fp8_ds_mla":
+        head_dim = MLA_FP8_DS_BYTES
+        if fmt == _lib.FMT_FP8:
+            fmt = _lib.FMT_RAW
+            _log_once("b200kv: the fp8_ds_mla cache already holds FP8 latent records: chunks are stored RAW")
+    hf = getattr(mc, "hf_text_config", None) or getattr(mc, "hf_config", None)
+    sparse = mla and hasattr(hf, "index_topk")   # vLLM's own test for a V3.2 model (deepseek_v2.py, is_v32)
     return KVGeometry(n_layers=mc.get_num_layers(pc), n_kv_heads=1 if mla else mc.get_num_kv_heads(pc),
-                      head_dim=mc.get_head_size(), n_blocks=n_blocks, block_tokens=cc.block_size,
-                      chunk_tokens=cfg.chunk_size, elem_bytes=elem, block_stride_bytes=0, fmt=cfg.fmt,
-                      layout=_lib.LAYOUT_MLA if mla else _lib.LAYOUT_NHD, dtype=dtype)
+                      head_dim=head_dim, n_blocks=n_blocks, block_tokens=cc.block_size,
+                      chunk_tokens=cfg.chunk_size, elem_bytes=elem, block_stride_bytes=0, fmt=fmt,
+                      layout=_lib.LAYOUT_MLA if mla else _lib.LAYOUT_NHD, dtype=dtype,
+                      idx_value_bytes=INDEXER_VALUE_BYTES if sparse else 0,
+                      idx_scale_bytes=INDEXER_SCALE_BYTES if sparse else 0)
+
+
+MLA_FP8_DS_BYTES = 656   # one token of vLLM's fp8_ds_mla latent cache (uint8): the FP8 latent record
+_LOGGED: set[str] = set()
+
+
+def _log_once(msg: str):
+    if msg not in _LOGGED:
+        _LOGGED.add(msg)
+        logger.info(msg)
 
 
 def owner_tag_of(instance_id: str) -> int:
@@ -159,6 +183,7 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
         self._pool = KVPool(self._pool_name, self.cfg.pool_bytes, geom.chunk_bytes, _lib.POOL_CREATE_OR_ATTACH)
         self._engine: KVEngine | None = None
         self._worker: WorkerState | None = None
+        self._wait_ahead, self._n_layers = False, 0   # layer-wise waits one layer ahead (register_kv_caches)
         self._sched: SchedulerState | None = None
         self._controller = None
         self._engine_id = str(ktc.engine_id or "engine")
@@ -209,7 +234,7 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
                 atexit.register(KVPool.unlink, self._pool_name)
         logger.info("b200kv connector role=%s kv_role=%s pool=%s (%.1f GB, chunk %d, fmt %s)",
                     role.name, self.kv_role, self._pool_name, self.cfg.max_local_cpu_size_gb, self._chunk,
-                    ("raw", "fp8", "q4")[self.cfg.fmt])
+                    ("raw", "fp8", "q4")[geometry_from_vllm(self._vllm_config, self.cfg).fmt])
 
     def _make_remote(self, key_seeds):
         """LMCACHE_REMOTE_URL=lm://host:port (deployment-vllm-multi.yaml:338-345): the cache-server
@@ -238,16 +263,23 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
     # ------------------------------------------------------------------ worker side
     def register_kv_caches(self, kv_caches: dict[str, torch.Tensor]):
         """KVConnectorBase_V1.register_kv_caches (base.py:251) — adapter :786-795."""
-        tensors = list(kv_caches.values())
-        if not tensors:
+        if not kv_caches:
             raise ValueError("no KV cache tensors to register")
+        # DeepSeek-V3.2: the latent layers and the indexer caches of the same layers come in one group
+        tensors, idx = split_indexer_caches(kv_caches)
         t0 = tensors[0]
         k, v, stride, nb, h, d, tile_layout = paged_layout_of(t0, self._block_size)
         geom0 = geometry_from_vllm(self._vllm_config, self.cfg)
         geom = KVGeometry(n_layers=len(tensors), n_kv_heads=h, head_dim=d, n_blocks=nb,
                           block_tokens=self._block_size, chunk_tokens=self._chunk,
-                          elem_bytes=t0.element_size(), block_stride_bytes=stride, fmt=self.cfg.fmt,
-                          layout=tile_layout, dtype=dtype_code(t0.dtype) or _lib.DTYPE_BF16)
+                          elem_bytes=t0.element_size(), block_stride_bytes=stride, fmt=geom0.fmt,
+                          layout=tile_layout, dtype=dtype_code(t0.dtype) or _lib.DTYPE_BF16,
+                          idx_value_bytes=INDEXER_VALUE_BYTES if idx else 0,
+                          idx_scale_bytes=INDEXER_SCALE_BYTES if idx else 0,
+                          idx_block_stride_bytes=idx[0].stride(0) if idx else 0)
+        if geom.indexed != geom0.indexed:
+            raise ValueError("KV cache tensors " + ("include" if idx else "lack") + " indexer caches, which the "
+                             "model config " + ("does not imply" if idx else "implies"))
         if geom.chunk_bytes != geom0.chunk_bytes:
             raise ValueError("KV cache tensors do not match the model geometry the pool was sized for "
                              f"({geom.chunk_bytes} vs {geom0.chunk_bytes} bytes per chunk)")
@@ -262,8 +294,15 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
                                 # per-engine pool lives on the GPU's own node
                                 numa_policy=_lib.NUMA_INTERLEAVE if self.cfg.pool_name else _lib.NUMA_LOCAL)
         logger.info("b200kv pool pages: %s", self._engine.numa_placement())
-        self._engine.register_kv_caches(tensors)
-        self._layer_index = {name: i for i, name in enumerate(kv_caches.keys())}
+        self._engine.register_kv_caches(kv_caches if idx else tensors)
+        # only the attention layers call wait_for_layer_load: the hook is keyed by the latent layers' names
+        lat_names = [n for n, t in kv_caches.items() if not any(t is x for x in idx)]
+        self._layer_index = {name: i for i, name in enumerate(lat_names)}
+        self._n_layers = len(lat_names)
+        # DeepSeek-V3.2 runs layer l's indexer, which reads the indexer keys of layer l, BEFORE layer l's attention
+        # calls wait_for_layer_load; the indexer calls no connector hook.  Layer-wise loads then wait one layer
+        # ahead: layer 0's group in start_load_kv, layer l+1's group in layer l's hook.
+        self._wait_ahead = geom.indexed
         self._layer_hooks_seen = 0
         self._worker = WorkerState(self._engine, self._block_size, self._chunk, self.kv_role,
                                    owner_tag=owner_tag_of(self.cfg.instance_id) if self.cfg.pool_name else 0,
@@ -331,11 +370,14 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
         full_graph = getattr(getattr(forward_context, "cudagraph_runtime_mode", None), "name", "NONE") == "FULL"
         self._worker.start_load(self._metas(), stream=stream,
                                 layers_per_group=self.cfg.layer_group if (self.cfg.layerwise and not full_graph) else 0)
+        if self._wait_ahead and self._worker.layer_loads:
+            self._worker.wait_layer(0, stream)     # layer 0's indexer runs before any hook
 
     def wait_for_layer_load(self, layer_name: str) -> None:
         """Chunk-wise loads are ordered before the forward pass by a stream wait.  Layer-wise loads
         (B200KV_LAYERWISE=1; LMCache `use_layerwise`, adapter :907-929): the compute stream waits
-        here, once per layer group, while later groups are still crossing PCIe."""
+        here, once per layer group, while later groups are still crossing PCIe.  With indexer caches (DeepSeek-V3.2)
+        the wait runs one layer ahead: the next layer's indexer reads its keys before that layer's hook runs."""
         w = self._worker
         if w is None or not w.layer_loads:
             return
@@ -343,8 +385,11 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
         if idx is None:
             return
         self._layer_hooks_seen += 1
-        if idx % self.cfg.layer_group == 0:
+        G = self.cfg.layer_group
+        if idx % G == 0:
             w.wait_layer(idx, torch.cuda.current_stream())
+        if self._wait_ahead and (idx + 1) % G == 0 and idx + 1 < self._n_layers:
+            w.wait_layer(idx + 1, torch.cuda.current_stream())
 
     def save_kv_layer(self, layer_name: str, kv_layer: torch.Tensor, attn_metadata, **kwargs: Any) -> None:
         return  # whole-request store in wait_for_save: CUDA-graph replay skips per-layer hooks (base.py:591-611)

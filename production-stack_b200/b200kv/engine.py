@@ -16,6 +16,7 @@ of being passed on every call.  Nothing here computes on the CPU: the data path 
 from __future__ import annotations
 
 import ctypes as C
+import re
 from dataclasses import dataclass
 
 import numpy as np
@@ -25,6 +26,9 @@ from ._lib import FMT_FP8, FMT_RAW, VARIANT_BULK, check, lib
 
 DEFAULT_SEED = 0x6232303030304B56  # keys are namespaced further by KVGeometry.key_seed()
 MLA_FP8_RECORD_BYTES = 656         # one (token, layer) of an MLA FP8 chunk (include/b200kv.h, B200KV_LAYOUT_MLA)
+# DeepSeek-V3.2's indexer key cache: per token 128 e4m3 values then, after the block's values, one fp32 scale
+# (vLLM's indexer_k_quant_and_cache; DeepseekV32IndexerCache has head_size 132)
+INDEXER_VALUE_BYTES, INDEXER_SCALE_BYTES = 128, 4
 
 
 def _as_i64(a) -> np.ndarray:
@@ -80,6 +84,11 @@ class KVGeometry:
     fmt: int = FMT_RAW
     layout: int = 0               # LAYOUT_NHD / LAYOUT_HND inside a block, or LAYOUT_MLA
     dtype: int = _lib.DTYPE_BF16  # element type of a 16-bit cache: DTYPE_BF16 or DTYPE_FP16 (b200kv_set_cache_dtype)
+    # indexer planes of an MLA model with sparse attention (DeepSeek-V3.2; b200kv_set_indexer): bytes of a token's
+    # values and of its scale in the split tile, and the planes' block stride (0 -> dense); 0 / 0 = none
+    idx_value_bytes: int = 0
+    idx_scale_bytes: int = 0
+    idx_block_stride_bytes: int = 0
 
     @property
     def fp16(self) -> bool:
@@ -88,8 +97,9 @@ class KVGeometry:
     @property
     def fmt_tag(self) -> int:
         """The format tag the engine records with every chunk (pool_fmt in b200kv_engine.cu): format, tile order
-        and cache element type.  bf16 tags are format | layout << 8, as before the element type was added."""
-        return self.fmt | (self.layout << 8) | (self.dtype << 16)
+        and cache element type, plus bit 24 with indexer planes.  bf16 tags are format | layout << 8, as before the
+        element type was added."""
+        return self.fmt | (self.layout << 8) | (self.dtype << 16) | (_lib.FMT_TAG_INDEXED if self.indexed else 0)
 
     @property
     def token_bytes(self) -> int:
@@ -98,6 +108,19 @@ class KVGeometry:
     @property
     def mla(self) -> bool:
         return self.layout == _lib.LAYOUT_MLA
+
+    @property
+    def indexed(self) -> bool:
+        """An indexer plane per layer next to the latent one (MLA with sparse attention)."""
+        return self.idx_value_bytes > 0
+
+    @property
+    def idx_token_bytes(self) -> int:
+        return self.idx_value_bytes + self.idx_scale_bytes
+
+    @property
+    def idx_stride(self) -> int:
+        return self.idx_block_stride_bytes or self.block_tokens * self.idx_token_bytes
 
     @property
     def planes(self) -> int:
@@ -113,13 +136,16 @@ class KVGeometry:
         worker_id, ...) — chunks of different models / shards / formats never alias.  An MLA latent is
         the same on every tensor-parallel rank, so its namespace keeps only the pipeline stage
         (rank // world_size) of the rank: one stored copy serves every rank of the stage.  An fp16 cache
-        appends "|fp16", so its chunks (RAW included) never alias a bf16 replica's; bf16 seeds are unchanged."""
+        appends "|fp16", so its chunks (RAW included) never alias a bf16 replica's; bf16 seeds are unchanged.  A
+        geometry with indexer planes appends "|idx<bytes per token>" (V3.2: "|idx132"); others are unchanged."""
         if self.mla:
             rank //= max(world_size, 1)
         tag = f"{model}|{world_size}|{rank}|{self.n_layers}|{self.n_kv_heads}|{self.head_dim}|" \
               f"{self.elem_bytes}|{self.chunk_tokens}|{self.fmt}|{self.layout}"
         if self.fp16:
             tag += "|fp16"
+        if self.indexed:
+            tag += f"|idx{self.idx_token_bytes}"
         return xxh64(tag.encode(), DEFAULT_SEED)
 
     def to_c(self, device: int, staging_bytes: int, owner: int, variant: int, stages: int,
@@ -132,16 +158,21 @@ class KVGeometry:
     @property
     def chunk_bytes(self) -> int:
         cfg = self.to_c(0, 0, 0, 0, 0, 0)
+        if self.indexed:
+            return check(int(lib().b200kv_engine_chunk_bytes_indexed(C.byref(cfg), self.idx_value_bytes,
+                                                                      self.idx_scale_bytes)),
+                         "b200kv_engine_chunk_bytes_indexed")
         return check(int(lib().b200kv_engine_chunk_bytes(C.byref(cfg))), "b200kv_engine_chunk_bytes")
 
     @property
     def payload_bytes_per_token(self) -> int:
         """Bytes one token occupies in a stored chunk (SURVEY.md §8d 'payload P')."""
         per = self.planes * self.token_bytes
+        idx = self.n_layers * self.idx_token_bytes   # indexer planes travel verbatim in every format
         if self.fmt == FMT_RAW:
-            return per
+            return per + idx
         if self.fmt == FMT_FP8:
-            return self.n_layers * MLA_FP8_RECORD_BYTES if self.mla else per // 2
+            return (self.n_layers * MLA_FP8_RECORD_BYTES + idx) if self.mla else per // 2
         return per * 9 // 32          # Q4: 4 bits + one bf16 scale per 32 elements = 4.5 bits per element
 
 
@@ -283,6 +314,44 @@ def _stream_ptr(stream) -> C.c_void_p:
     return C.c_void_p(int(stream))
 
 
+def indexer_layout_of(t, block_tokens: int, token_bytes: int = INDEXER_VALUE_BYTES + INDEXER_SCALE_BYTES):
+    """(ptr, block_stride_bytes, n_blocks) of one layer's indexer key cache: (NB, bs, 132) uint8 as vLLM's
+    DeepseekV32IndexerBackend.get_kv_cache_shape allocates it, a block holding [bs][128] values then [bs][4] scales."""
+    if t.dim() != 3 or t.element_size() != 1 or t.shape[1] != block_tokens or t.shape[2] != token_bytes:
+        raise ValueError(f"indexer cache shape {tuple(t.shape)} / {t.dtype} is not (NB, {block_tokens}, {token_bytes}) bytes")
+    if tuple(t.stride()[1:]) != (token_bytes, 1) or t.stride(0) < block_tokens * token_bytes:
+        raise NotImplementedError("unsupported order inside an indexer block (strides %s)" % (tuple(t.stride()),))
+    return t.data_ptr(), t.stride(0), t.shape[0]
+
+
+def _layer_number(name: str):
+    m = re.search(r"\.(\d+)\.", f".{name}.")
+    return int(m.group(1)) if m else None
+
+
+def split_indexer_caches(kv_caches, token_bytes: int = INDEXER_VALUE_BYTES + INDEXER_SCALE_BYTES):
+    """kv_caches (dict name -> tensor, or a list) -> (latent tensors, indexer tensors), each in layer order.  vLLM
+    puts a DeepSeek-V3.2's latent layers and its DeepseekV32IndexerCache layers in one KV-cache group, so
+    register_kv_caches gets both.  An indexer cache is a rank-3 one-byte tensor of `token_bytes` per token (V3.2:
+    132), which no latent cache is (576 elements, or 656 bytes with fp8_ds_mla).  With names, the split must
+    also agree with them ("indexer" in a name), and the i-th latent and i-th indexer tensor must be the same
+    layer.  Without any indexer tensor the second list is empty."""
+    items = list(kv_caches.items()) if isinstance(kv_caches, dict) else [(None, t) for t in kv_caches]
+    lat, idx = [], []
+    for name, t in items:
+        is_idx = t.dim() == 3 and t.element_size() == 1 and t.shape[-1] == token_bytes
+        if name is not None and ("indexer" in name) != is_idx:
+            raise ValueError(f"KV cache {name}: shape {tuple(t.shape)} / {t.dtype} contradicts its layer name")
+        (idx if is_idx else lat).append((name, t))
+    if idx:
+        if len(idx) != len(lat):
+            raise ValueError(f"{len(lat)} latent and {len(idx)} indexer caches: need one of each per layer")
+        for (nl, _), (ni, _) in zip(lat, idx):
+            if nl is not None and _layer_number(nl) != _layer_number(ni):
+                raise ValueError(f"latent cache {nl} and indexer cache {ni} are not the same layer")
+    return [t for _, t in lat], [t for _, t in idx]
+
+
 def paged_layout_of(t, block_tokens: int, layout: str | None = None):
     """(k_ptr, v_ptr, block_stride_bytes, n_blocks, H, D, tile_layout) of one layer's paged KV tensor.
     FlashAttention (2, NB, bs, H, D) (vllm/v1/attention/backends/flash_attn.py:140-149) or
@@ -338,21 +407,30 @@ class KVEngine:
         self._kv_refs = None
         if geom.fp16:
             self.set_cache_dtype(_lib.DTYPE_FP16)
+        if geom.indexed:
+            self.set_indexer(geom.idx_value_bytes, geom.idx_scale_bytes, geom.idx_stride)
 
     def set_cache_dtype(self, dtype: int):
         """b200kv_set_cache_dtype: legal before registration only (-EBUSY after)."""
         check(lib().b200kv_set_cache_dtype(self._h, dtype), "b200kv_set_cache_dtype")
 
+    def set_indexer(self, value_bytes: int, scale_bytes: int, block_stride: int):
+        """b200kv_set_indexer: an indexer plane per layer on an MLA engine; before registration only (-EBUSY after)."""
+        check(lib().b200kv_set_indexer(self._h, value_bytes, scale_bytes, C.c_uint64(block_stride)),
+              "b200kv_set_indexer")
+
     # ---- registration ---------------------------------------------------------------------
     def _plane_ptrs(self, k_ptrs, v_ptrs):
-        """ctypes arrays of the K and V pointers; MLA takes one latent pointer per layer and v_ptrs None."""
+        """ctypes arrays of the K and V pointers; MLA takes one latent pointer per layer and v_ptrs None, or the
+        indexer planes in v_ptrs when the geometry has them."""
         L = self.geom.n_layers
-        if self.geom.mla:
+        if self.geom.mla and not self.geom.indexed:
             if len(k_ptrs) != L or v_ptrs is not None:
                 raise ValueError("MLA: need one latent pointer per layer and no V pointers")
             return (C.c_void_p * L)(*[C.c_void_p(int(p)) for p in k_ptrs]), None
         if len(k_ptrs) != L or v_ptrs is None or len(v_ptrs) != L:
-            raise ValueError("need one K and one V pointer per layer")
+            raise ValueError("need one latent and one indexer pointer per layer" if self.geom.mla
+                             else "need one K and one V pointer per layer")
         return ((C.c_void_p * L)(*[C.c_void_p(int(p)) for p in k_ptrs]),
                 (C.c_void_p * L)(*[C.c_void_p(int(p)) for p in v_ptrs]))
 
@@ -361,8 +439,21 @@ class KVEngine:
         check(lib().b200kv_register_kv(self._h, ka, va), "b200kv_register_kv")
 
     def register_kv_caches(self, kv_caches, layout: str | None = None):
-        """kv_caches: list (or dict values) of per-layer torch tensors on this device."""
+        """kv_caches: list (or dict) of per-layer torch tensors on this device.  With indexer planes, the latent and
+        indexer caches of every layer (split_indexer_caches tells them apart)."""
         tensors = list(kv_caches.values()) if isinstance(kv_caches, dict) else list(kv_caches)
+        idx_ptrs = None
+        if self.geom.indexed:
+            lat, idx = split_indexer_caches(kv_caches, self.geom.idx_token_bytes)
+            if not idx:
+                raise ValueError("the engine has indexer planes but no indexer cache was given")
+            idx_ptrs = []
+            for t in idx:
+                ptr, stride, nb = indexer_layout_of(t, self.geom.block_tokens, self.geom.idx_token_bytes)
+                if stride != self.geom.idx_stride or nb < self.geom.n_blocks:
+                    raise ValueError("indexer cache tensor does not match the engine geometry")
+                idx_ptrs.append(ptr)
+            tensors_all, tensors = tensors, lat
         ks, vs = [], []
         for t in tensors:
             k, v, stride, nb, h, d, tl = paged_layout_of(t, self.geom.block_tokens, layout)
@@ -377,8 +468,8 @@ class KVEngine:
                                  f"({'float16' if self.geom.fp16 else 'bfloat16'})")
             ks.append(k)
             vs.append(v)
-        self._kv_refs = tensors  # keep the storage alive
-        self.register_kv_ptrs(ks, None if self.geom.mla else vs)
+        self._kv_refs = tensors if idx_ptrs is None else tensors_all  # keep the storage alive
+        self.register_kv_ptrs(ks, idx_ptrs if self.geom.mla else vs)
 
     # ---- LMCache-shaped data path ---------------------------------------------------------
     def _keys(self, tokens) -> np.ndarray:
@@ -549,14 +640,14 @@ class KVEngine:
                                           _stream_ptr(stream)), "b200kv_scatter_chunks")
 
     def export_ipc(self) -> bytes:
-        n = self.geom.planes
+        n = self.geom.planes + (self.geom.n_layers if self.geom.indexed else 0)
         arr = (_lib.IpcDesc * n)()
         check(lib().b200kv_export_ipc(self._h, arr, n), "b200kv_export_ipc")
         return bytes(arr)
 
     def import_peer(self, peer_id: int, peer_device: int, descs: bytes,
                     peer_block_stride: int | None = None, peer_n_blocks: int | None = None):
-        n = self.geom.planes
+        n = self.geom.planes + (self.geom.n_layers if self.geom.indexed else 0)
         arr = (_lib.IpcDesc * n).from_buffer_copy(descs)
         check(lib().b200kv_import_peer(self._h, peer_id, peer_device, arr, n,
                                         peer_block_stride or self.geom.stride,

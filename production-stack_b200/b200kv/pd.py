@@ -78,12 +78,18 @@ def _dtype_of(geom) -> int:
     return int(getattr(geom, "dtype", DTYPE_BF16))
 
 
+def _indexer_of(geom) -> int:
+    """Bytes per token of a geometry's indexer planes (KVGeometry.idx_token_bytes; 0 = none)."""
+    return int(getattr(geom, "idx_token_bytes", 0))
+
+
 def publish_ipc(engine_id: str, engine, device: int, rank: int = 0, tp_size: int = 1) -> str:
     g = engine.geom
     doc = {"engine_id": engine_id, "device": device, "pid": os.getpid(), "rank": rank, "tp_size": tp_size,
            "n_blocks": g.n_blocks,
            "block_stride": g.stride, "n_layers": g.n_layers, "n_kv_heads": g.n_kv_heads, "head_dim": g.head_dim,
            "block_tokens": g.block_tokens, "elem_bytes": g.elem_bytes, "layout": g.layout, "dtype": _dtype_of(g),
+           "indexer": _indexer_of(g),
            "descs": base64.b64encode(engine.export_ipc()).decode()}
     path = ipc_path(engine_id, rank)
     tmp = path + f".{os.getpid()}.tmp"
@@ -133,9 +139,10 @@ class PeerResolver:
                              f"differs from local {self.rank}/{self.tp_size}")
         g = self.engine.geom
         doc.setdefault("dtype", DTYPE_BF16)   # documents published before the field are bf16 caches
+        doc.setdefault("indexer", 0)          # ... and caches without indexer planes
         for k, mine in (("n_layers", g.n_layers), ("n_kv_heads", g.n_kv_heads), ("head_dim", g.head_dim),
                         ("block_tokens", g.block_tokens), ("elem_bytes", g.elem_bytes), ("layout", g.layout),
-                        ("dtype", _dtype_of(g))):
+                        ("dtype", _dtype_of(g)), ("indexer", _indexer_of(g))):
             if doc[k] != mine:
                 raise ValueError(f"peer {remote_engine_id}: {k}={doc[k]} differs from local {mine}")
         pid = len(self.ids)

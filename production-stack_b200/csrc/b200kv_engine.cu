@@ -133,6 +133,7 @@ struct Peer {
   bool valid = false;
   int device = -1;
   uint64_t* d_bases = nullptr;
+  uint64_t* d_idx_bases = nullptr;   // indexer planes (engines with b200kv_set_indexer); same block stride as ours
   uint64_t block_stride = 0;
   uint64_t n_blocks = 0;
   std::vector<void*> opened;  // cudaIpcOpenMemHandle mappings to close
@@ -151,6 +152,13 @@ struct Geometry {
   bool mla;               // one latent plane per layer (B200KV_LAYOUT_MLA)
   uint32_t row_bytes;     // D*elem
   uint32_t dtype;         // B200KV_DTYPE_*: element type of the cache (b200kv_set_cache_dtype; bf16 by default)
+  // indexer planes (MLA with sparse attention, b200kv_set_indexer): one split tile per block, [bs][idx_vb] values
+  // then [bs][idx_sb] scales; in a chunk, L slabs of [C][idx_vb] + [C][idx_sb] after the latent part
+  bool indexed;
+  uint32_t idx_vb, idx_sb;
+  uint64_t idx_stride;    // bytes between consecutive blocks of one indexer plane
+  uint64_t idx_off;       // where the indexer slabs start inside a chunk
+  uint64_t idx_slab;      // C * (idx_vb + idx_sb): one layer's indexer slab
 };
 
 int make_geometry(const b200kv_engine_config* c, Geometry* g) {
@@ -175,6 +183,9 @@ int make_geometry(const b200kv_engine_config* c, Geometry* g) {
   g->row_bytes = g->D * g->elem;
   g->dtype = B200KV_DTYPE_BF16;
   g->scales_bytes = 0;
+  g->indexed = false;
+  g->idx_vb = g->idx_sb = 0;
+  g->idx_stride = g->idx_off = g->idx_slab = 0;
   if (g->token_bytes % 16) return B200KV_EINVAL;  // 16-byte vectors / bulk-copy granularity
   if (g->hnd && g->row_bytes % 16) return B200KV_EINVAL;
   if (c->format == B200KV_FMT_RAW) {
@@ -213,6 +224,27 @@ int make_geometry(const b200kv_engine_config* c, Geometry* g) {
   return B200KV_OK;
 }
 
+// Adds an indexer plane per layer to an MLA geometry (b200kv_set_indexer): the chunk becomes the latent part as
+// before, unrounded, followed by L indexer slabs, and the whole is rounded up to 256 bytes.
+int add_indexer(Geometry* g, int64_t value_bytes, int64_t scale_bytes, uint64_t block_stride) {
+  if (!g->mla || g->scales_bytes) return B200KV_EINVAL;
+  if (value_bytes <= 0 || value_bytes % 16 || value_bytes > (1 << 16) || scale_bytes <= 0 || scale_bytes % 4 ||
+      scale_bytes > (1 << 16))
+    return B200KV_EINVAL;
+  const uint64_t tile = static_cast<uint64_t>(g->bs) * static_cast<uint64_t>(value_bytes + scale_bytes);
+  if (block_stride < tile || block_stride % 16) return B200KV_EINVAL;
+  const uint64_t slab = static_cast<uint64_t>(g->C) * static_cast<uint64_t>(value_bytes + scale_bytes);
+  if (slab % 16) return B200KV_EINVAL;   // every slab starts on a 16-byte boundary (bulk copies)
+  g->indexed = true;
+  g->idx_vb = static_cast<uint32_t>(value_bytes);
+  g->idx_sb = static_cast<uint32_t>(scale_bytes);
+  g->idx_stride = block_stride;
+  g->idx_off = g->slab_bytes * g->planes;
+  g->idx_slab = slab;
+  g->chunk_bytes = (g->idx_off + g->idx_slab * g->L + 255) / 256 * 256;
+  return B200KV_OK;
+}
+
 // The geometry kv_fp8_store3_kernel needs: a (chunk, head) unit of bf16 fits one consumer group's registers, a
 // row is a whole number of 16-byte vectors that divides the group, one block's rows of a head fill whole 128-byte
 // lines, a chunk has at most 256 blocks, and (HND) one step of the group's tokens is whole tiles.
@@ -238,6 +270,7 @@ struct b200kv_ctx {
   cudaStream_t s_gather = nullptr, s_d2h = nullptr, s_h2d = nullptr, s_scatter = nullptr;
   cudaEvent_t fence = nullptr;          // stream_wait's event
   uint64_t* d_bases = nullptr;
+  uint64_t* d_idx_bases = nullptr;      // [L] indexer planes (g.indexed)
   bool kv_registered = false;
   std::vector<const void*> h_k, h_v;
 
@@ -407,11 +440,12 @@ BulkKernel bulk_kernel(int S, int LAG) {
   }
 }
 
-// format tag recorded with a chunk: a pool shared by engines of different tile order, codec or cache element
-// type never hands one engine's bytes to another (bf16 engines keep the tags they had before the dtype field)
+// format tag recorded with a chunk: a pool shared by engines of different tile order, codec, cache element type or
+// indexer planes never hands one engine's bytes to another (bf16 engines keep the tags they had before the dtype
+// field, engines without indexer planes the tags they had before bit 24)
 uint32_t pool_fmt(const b200kv_ctx* ctx) {
   return static_cast<uint32_t>(ctx->cfg.format) | (static_cast<uint32_t>(ctx->cfg.kv_layout) << 8) |
-         (ctx->g.dtype << 16);
+         (ctx->g.dtype << 16) | (ctx->g.indexed ? 1u << 24 : 0u);
 }
 
 PagedSide local_side(const b200kv_ctx* ctx) {
@@ -520,6 +554,11 @@ int launch_per_run(b200kv_ctx* ctx, CopyMode mode, const TableView& tv, size_t f
   return launched(ctx);
 }
 
+// dynamic shared memory of kv_indexer_copy_kernel: the warps' mbarriers and stages
+size_t indexer_smem_bytes(const Geometry& g) {
+  return kIdxBarBytes + static_cast<size_t>(kIdxWarps) * ((static_cast<size_t>(g.bs) * (g.idx_vb + g.idx_sb) + 15) & ~15ull);
+}
+
 // FP8 latent records of an MLA engine, either direction, runs [f0, f0 + nf): one warp per (run, plane) unit.
 template <int DT>
 int launch_mla_fp8(b200kv_ctx* ctx, CopyMode mode, const TableView& tv, size_t f0, size_t nf, cudaStream_t s,
@@ -543,11 +582,51 @@ int launch_lossy(b200kv_ctx* ctx, CopyMode mode, const OpTable& t, const TableVi
   return launch_per_run<DT>(ctx, mode, tv, f0, nf, s, pb, np);
 }
 
+// The indexer planes of layers [pb, pb + np) (np == 0: every layer) of runs [f0, f0 + nf), verbatim in every
+// direction.  KernelArgs carry the indexer side in the fields kv_indexer_copy_kernel names.
+int launch_indexer(b200kv_ctx* ctx, CopyMode mode, const TableView& tv, size_t f0, size_t nf, cudaStream_t s,
+                   uint32_t pb, uint32_t np, const Peer* peer) {
+  const Geometry& g = ctx->g;
+  KernelArgs a = kernel_args(ctx, tv, f0, pb, np, peer);
+  a.paged.bases = ctx->d_idx_bases;
+  a.paged.block_stride = g.idx_stride;
+  a.paged.token_bytes = g.idx_vb;
+  a.peer = a.paged;
+  if (peer) a.peer.bases = peer->d_idx_bases;
+  a.chunk.slab_bytes = g.idx_slab;
+  a.chunk.scales_off = g.idx_off;
+  a.chunk.token_bytes = g.idx_vb;
+  a.row_bytes = g.idx_sb;
+  a.total_units = static_cast<uint32_t>(nf) * a.n_planes;
+  const uint32_t grid = std::min<uint32_t>((a.total_units + kIdxWarps - 1) / kIdxWarps,
+                                           static_cast<uint32_t>(ctx->sm_count) * 8u);
+  if (grid == 0) return B200KV_OK;
+  const size_t smem = indexer_smem_bytes(g);
+  switch (mode) {
+    case kStore: kv_indexer_copy_kernel<kStore><<<grid, kIdxWarps * 32, smem, s>>>(a); break;
+    case kLoad: kv_indexer_copy_kernel<kLoad><<<grid, kIdxWarps * 32, smem, s>>>(a); break;
+    default: kv_indexer_copy_kernel<kPull><<<grid, kIdxWarps * 32, smem, s>>>(a); break;
+  }
+  return launched(ctx);
+}
+
 // Launches the kernels that move chunks [c0, c1) of table t, planes [pb, pb + np) (np == 0: every plane), in
-// direction `mode`.  A pull copies pages to pages whatever the chunk format.  The FP8 store of a K/V engine always
-// takes the whole table.
+// direction `mode`, and then, on an engine with indexer planes, the indexer planes of the same layers.
+int launch_planes(b200kv_ctx* ctx, CopyMode mode, const OpTable& t, const TableView& tv, uint32_t c0, uint32_t c1,
+                  cudaStream_t s, uint32_t pb, uint32_t np, const Peer* peer);
+
 int launch_op(b200kv_ctx* ctx, CopyMode mode, const OpTable& t, const TableView& tv, uint32_t c0, uint32_t c1,
               cudaStream_t s, uint32_t pb = 0, uint32_t np = 0, const Peer* peer = nullptr) {
+  const int rc = launch_planes(ctx, mode, t, tv, c0, c1, s, pb, np, peer);
+  if (rc || !ctx->g.indexed) return rc;
+  const size_t f0 = t.full_off[c0], nf = t.full_off[c1] - f0;   // MLA tables have full runs only
+  return launch_indexer(ctx, mode, tv, f0, nf, s, pb, np, peer);
+}
+
+// The latent (or K and V) planes of launch_op.  A pull copies pages to pages whatever the chunk format.  The FP8
+// store of a K/V engine always takes the whole table.
+int launch_planes(b200kv_ctx* ctx, CopyMode mode, const OpTable& t, const TableView& tv, uint32_t c0, uint32_t c1,
+                  cudaStream_t s, uint32_t pb, uint32_t np, const Peer* peer) {
   const size_t f0 = t.full_off[c0], nf = t.full_off[c1] - f0;
   const int fmt = mode == kPull ? B200KV_FMT_RAW : ctx->cfg.format;
   if (fmt != B200KV_FMT_RAW)
@@ -564,6 +643,7 @@ int launch_op(b200kv_ctx* ctx, CopyMode mode, const OpTable& t, const TableView&
 // Planes [pb, pb + np) of one chunk between the pinned pool and staging; np == 0 moves the whole chunk, as
 // one copy of chunk_bytes when the chunk is full.  Partial chunks move only their tokens.  The FP8 scales
 // travel with a whole chunk, and with a plane range when `with_scales` (the first group of a layer-wise load).
+// Indexer slabs travel with their layers.
 int copy_chunk_planes(b200kv_ctx* ctx, void* dst, const void* src, uint32_t n_tok, cudaMemcpyKind kind,
                       cudaStream_t s, uint32_t pb = 0, uint32_t np = 0, bool with_scales = true) {
   const Geometry& g = ctx->g;
@@ -586,6 +666,20 @@ int copy_chunk_planes(b200kv_ctx* ctx, void* dst, const void* src, uint32_t n_to
     CU_TRY(cudaMemcpyAsync(static_cast<uint8_t*>(dst) + g.scales_off, static_cast<const uint8_t*>(src) + g.scales_off,
                            g.scales_bytes, kind, s));
     moved += g.scales_bytes;
+  }
+  if (g.indexed && !whole) {   // the indexer slabs of the same layers (MLA: plane == layer)
+    uint8_t* di = static_cast<uint8_t*>(dst) + g.idx_off + static_cast<uint64_t>(pb) * g.idx_slab;
+    const uint8_t* si = static_cast<const uint8_t*>(src) + g.idx_off + static_cast<uint64_t>(pb) * g.idx_slab;
+    if (n_tok == g.C) {
+      CU_TRY(cudaMemcpyAsync(di, si, static_cast<uint64_t>(np) * g.idx_slab, kind, s));
+      moved += static_cast<uint64_t>(np) * g.idx_slab;
+    } else {   // the values of the chunk's tokens, then their scales
+      const uint64_t sc = static_cast<uint64_t>(g.C) * g.idx_vb;
+      CU_TRY(cudaMemcpy2DAsync(di, g.idx_slab, si, g.idx_slab, static_cast<size_t>(n_tok) * g.idx_vb, np, kind, s));
+      CU_TRY(cudaMemcpy2DAsync(di + sc, g.idx_slab, si + sc, g.idx_slab, static_cast<size_t>(n_tok) * g.idx_sb, np,
+                               kind, s));
+      moved += static_cast<uint64_t>(n_tok) * (g.idx_vb + g.idx_sb) * np;
+    }
   }
   if (kind == cudaMemcpyDeviceToHost) ctx->stats.d2h_bytes += moved;
   else ctx->stats.h2d_bytes += moved;
@@ -632,6 +726,19 @@ extern "C" int64_t b200kv_engine_chunk_bytes(const b200kv_engine_config* cfg) {
   if (!cfg) return B200KV_EINVAL;
   Geometry g;
   const int rc = make_geometry(cfg, &g);
+  if (rc) return rc;
+  return static_cast<int64_t>(g.chunk_bytes);
+}
+
+extern "C" int64_t b200kv_engine_chunk_bytes_indexed(const b200kv_engine_config* cfg, int32_t value_bytes,
+                                                    int32_t scale_bytes) {
+  if (!cfg) return B200KV_EINVAL;
+  Geometry g;
+  int rc = make_geometry(cfg, &g);
+  if (rc) return rc;
+  // the block stride does not enter the chunk: pass the smallest legal one
+  rc = add_indexer(&g, value_bytes, scale_bytes,
+                   (static_cast<uint64_t>(g.bs) * static_cast<uint64_t>(std::max(value_bytes + scale_bytes, 0)) + 15) / 16 * 16);
   if (rc) return rc;
   return static_cast<int64_t>(g.chunk_bytes);
 }
@@ -756,6 +863,36 @@ extern "C" int b200kv_engine_create(const b200kv_engine_config* cfg, b200kv_pool
   return B200KV_OK;
 }
 
+// The staging ring: as many chunk_bytes slots as staging_bytes holds.  The new ring is built completely before it
+// replaces the engine's current one (b200kv_set_indexer re-cuts the ring for its larger chunk before any op has used
+// it), so a refusal or a failed allocation leaves the engine with the ring it had.
+static int make_staging(b200kv_ctx* ctx, uint64_t chunk_bytes) {
+  const uint64_t n_stage = ctx->cfg.staging_bytes / chunk_bytes;
+  if (ctx->pool && n_stage < 2) return B200KV_EINVAL;  // store/load need one staging chunk each
+  uint8_t* buf = nullptr;
+  std::vector<StageSlot> ring(n_stage);
+  if (n_stage > 0) {
+    cudaError_t e = cudaMalloc(&buf, n_stage * chunk_bytes);
+    for (size_t i = 0; e == cudaSuccess && i < ring.size(); ++i)
+      e = cudaEventCreateWithFlags(&ring[i].free_ev, cudaEventDisableTiming);
+    if (e != cudaSuccess) {
+      set_err("staging ring", e, __LINE__);
+      for (auto& r : ring)
+        if (r.free_ev) cudaEventDestroy(r.free_ev);
+      if (buf) cudaFree(buf);
+      return B200KV_ENODEV;
+    }
+  }
+  for (auto& r : ctx->stage)
+    if (r.free_ev) cudaEventDestroy(r.free_ev);
+  if (ctx->d_staging) cudaFree(ctx->d_staging);
+  ctx->d_staging = buf;
+  ctx->stage = std::move(ring);
+  ctx->n_store_slots = static_cast<uint32_t>(n_stage / 2);
+  ctx->store_next = ctx->load_next = 0;
+  return B200KV_OK;
+}
+
 static int engine_create_impl(const b200kv_engine_config* cfg, b200kv_pool* pool, b200kv_ctx** out) {
   Geometry g;
   int rc = make_geometry(cfg, &g);
@@ -831,16 +968,8 @@ static int engine_create_impl(const b200kv_engine_config* cfg, b200kv_pool* pool
 
   CU_TRY(cudaMalloc(&ctx->d_bases, sizeof(uint64_t) * g.planes));
 
-  const uint64_t n_stage = cfg->staging_bytes / g.chunk_bytes;
-  if (n_stage > 0) {
-    CU_TRY(cudaMalloc(&ctx->d_staging, n_stage * g.chunk_bytes));
-    ctx->stage.resize(n_stage);
-    for (auto& s : ctx->stage) CU_TRY(cudaEventCreateWithFlags(&s.free_ev, cudaEventDisableTiming));
-    if (pool && n_stage < 2) return B200KV_EINVAL;  // one half each for stores and loads
-    ctx->n_store_slots = static_cast<uint32_t>(n_stage / 2);
-  } else if (pool) {
-    return B200KV_EINVAL;  // store/load need at least one staging chunk
-  }
+  rc = make_staging(ctx, g.chunk_bytes);
+  if (rc) return rc;
   for (auto& t : ctx->tables) {
     CU_TRY(cudaHostAlloc(&t.host, kTableBytes, cudaHostAllocDefault));
     CU_TRY(cudaMalloc(&t.dev, kTableBytes));
@@ -893,6 +1022,7 @@ extern "C" int b200kv_engine_destroy(b200kv_ctx* ctx) {
     if (!p.valid) continue;
     for (void* m : p.opened) cudaIpcCloseMemHandle(m);
     cudaFree(p.d_bases);
+    if (p.d_idx_bases) cudaFree(p.d_idx_bases);
   }
   for (auto& t : ctx->tables) {
     if (t.host) cudaFreeHost(t.host);
@@ -911,6 +1041,7 @@ extern "C" int b200kv_engine_destroy(b200kv_ctx* ctx) {
   for (void* m : ctx->tier_imports) cudaIpcCloseMemHandle(m);
   if (ctx->tier_base) cudaFree(ctx->tier_base);
   if (ctx->d_bases) cudaFree(ctx->d_bases);
+  if (ctx->d_idx_bases) cudaFree(ctx->d_idx_bases);
   if (ctx->d_tmaps) cudaFree(ctx->d_tmaps);
   if (ctx->fence) cudaEventDestroy(ctx->fence);
   for (cudaStream_t s : {ctx->s_gather, ctx->s_d2h, ctx->s_h2d, ctx->s_scatter})
@@ -978,10 +1109,42 @@ extern "C" int b200kv_set_cache_dtype(b200kv_ctx* ctx, int32_t dtype) {
   return B200KV_OK;
 }
 
+extern "C" int b200kv_set_indexer(b200kv_ctx* ctx, int32_t value_bytes, int32_t scale_bytes,
+                                  uint64_t block_stride_bytes) {
+  if (!ctx) return B200KV_EINVAL;
+  DeviceGuard dg(ctx->cfg.device);
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  if (ctx->kv_registered || ctx->tier_base) return B200KV_EBUSY;   // pages or tier slots sized without the planes
+  if (!ctx->g.mla) return B200KV_EINVAL;
+  Geometry g;
+  int rc = make_geometry(&ctx->cfg, &g);
+  if (rc) return rc;
+  g.dtype = ctx->g.dtype;
+  rc = add_indexer(&g, value_bytes, scale_bytes, block_stride_bytes);
+  if (rc) return rc;
+  // everything that can refuse is checked before the staging ring is rebuilt
+  if (indexer_smem_bytes(g) > 227u * 1024) return B200KV_ENOTSUP;
+  const uint64_t n_stage = ctx->cfg.staging_bytes / g.chunk_bytes;
+  if (ctx->pool) {
+    b200kv_pool_stats ps;
+    b200kv_pool_get_stats(ctx->pool, &ps);
+    if (ps.slot_bytes < g.chunk_bytes || n_stage < 2) return B200KV_EINVAL;
+  }
+  typedef void (*IndexerKernel)(KernelArgs);
+  for (IndexerKernel k : {kv_indexer_copy_kernel<kStore>, kv_indexer_copy_kernel<kLoad>, kv_indexer_copy_kernel<kPull>})
+    CU_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(indexer_smem_bytes(g))));
+  if (!ctx->d_idx_bases) CU_TRY(cudaMalloc(&ctx->d_idx_bases, sizeof(uint64_t) * g.L));
+  rc = make_staging(ctx, g.chunk_bytes);   // the engine keeps its geometry and ring if this fails
+  if (rc) return rc;
+  ctx->g = g;
+  return B200KV_OK;
+}
+
 extern "C" int b200kv_register_kv(b200kv_ctx* ctx, const void* const* k_ptrs,
                                   const void* const* v_ptrs) {
   const uint32_t ppl = ctx ? ctx->g.planes_per_layer : 0;
-  if (!ctx || !k_ptrs || (ppl == 2) != (v_ptrs != nullptr)) return B200KV_EINVAL;   // MLA: v_ptrs NULL
+  // MLA: v_ptrs NULL, or the indexer planes on an engine with b200kv_set_indexer
+  if (!ctx || !k_ptrs || (ppl == 2 || ctx->g.indexed) != (v_ptrs != nullptr)) return B200KV_EINVAL;
   DeviceGuard dg(ctx->cfg.device);
   std::lock_guard<std::mutex> lk(ctx->mu);
   std::vector<uint64_t> h(ctx->g.planes);
@@ -993,6 +1156,14 @@ extern "C" int b200kv_register_kv(b200kv_ctx* ctx, const void* const* k_ptrs,
       if (!p || p % 16) return B200KV_EINVAL;
       h[ppl * l + kv] = p;
     }
+  }
+  if (ctx->g.indexed) {
+    std::vector<uint64_t> hi(ctx->g.L);
+    for (uint32_t l = 0; l < ctx->g.L; ++l) {
+      hi[l] = reinterpret_cast<uint64_t>(v_ptrs[l]);
+      if (!hi[l] || hi[l] % 16) return B200KV_EINVAL;
+    }
+    CU_TRY(cudaMemcpy(ctx->d_idx_bases, hi.data(), sizeof(uint64_t) * hi.size(), cudaMemcpyHostToDevice));
   }
   CU_TRY(cudaMemcpy(ctx->d_bases, h.data(), sizeof(uint64_t) * h.size(), cudaMemcpyHostToDevice));
   build_tensor_maps(ctx, h);
@@ -1502,9 +1673,12 @@ extern "C" int b200kv_wait_all(b200kv_ctx* ctx) {
 // ------------------------------------------------------------------------------------------------
 // peers
 // ------------------------------------------------------------------------------------------------
+// IPC descriptors of an engine's planes: K and V (2L), latent (L), or latent and indexer (2L) planes
+static uint32_t n_descs_of(const Geometry& g) { return g.planes + (g.indexed ? g.L : 0u); }
+
 extern "C" int b200kv_export_ipc(b200kv_ctx* ctx, b200kv_ipc_desc* descs_out, int32_t n_descs) {
   if (!ctx || !descs_out) return B200KV_EINVAL;
-  if (!ctx->kv_registered || n_descs != static_cast<int32_t>(ctx->g.planes)) return B200KV_EINVAL;
+  if (!ctx->kv_registered || n_descs != static_cast<int32_t>(n_descs_of(ctx->g))) return B200KV_EINVAL;
   DeviceGuard dg(ctx->cfg.device);
   typedef CUresult (*GetRange)(CUdeviceptr*, size_t*, CUdeviceptr);
   void* fn = nullptr;
@@ -1513,12 +1687,12 @@ extern "C" int b200kv_export_ipc(b200kv_ctx* ctx, b200kv_ipc_desc* descs_out, in
   if (!fn || qr != cudaDriverEntryPointSuccess) return B200KV_ENODEV;
   GetRange get_range = reinterpret_cast<GetRange>(fn);
   for (uint32_t l = 0; l < ctx->g.L; ++l) {
-    for (uint32_t kv = 0; kv < ctx->g.planes_per_layer; ++kv) {
+    for (uint32_t kv = 0; kv < n_descs_of(ctx->g) / ctx->g.L; ++kv) {
       const void* p = kv ? ctx->h_v[l] : ctx->h_k[l];
       CUdeviceptr base = 0;
       size_t size = 0;
       if (get_range(&base, &size, reinterpret_cast<CUdeviceptr>(p)) != CUDA_SUCCESS) return B200KV_ENODEV;
-      b200kv_ipc_desc& d = descs_out[kv * ctx->g.L + l];  // K planes then V planes (MLA: latent planes)
+      b200kv_ipc_desc& d = descs_out[kv * ctx->g.L + l];  // K planes then V planes (MLA: latent, then indexer planes)
       std::memset(&d, 0, sizeof(d));
       cudaIpcMemHandle_t h;
       CU_TRY(cudaIpcGetMemHandle(&h, reinterpret_cast<void*>(base)));
@@ -1533,11 +1707,15 @@ extern "C" int b200kv_export_ipc(b200kv_ctx* ctx, b200kv_ipc_desc* descs_out, in
 
 static int install_peer(b200kv_ctx* ctx, int32_t peer_id, int32_t peer_device,
                         const std::vector<uint64_t>& bases, uint64_t stride, uint64_t n_blocks,
-                        std::vector<void*>&& opened) {
+                        std::vector<void*>&& opened, const std::vector<uint64_t>& idx_bases = {}) {
   Peer& p = ctx->peers[peer_id];
   if (p.valid) return B200KV_EEXIST;
   CU_TRY(cudaMalloc(&p.d_bases, sizeof(uint64_t) * bases.size()));
   CU_TRY(cudaMemcpy(p.d_bases, bases.data(), sizeof(uint64_t) * bases.size(), cudaMemcpyHostToDevice));
+  if (!idx_bases.empty()) {
+    CU_TRY(cudaMalloc(&p.d_idx_bases, sizeof(uint64_t) * idx_bases.size()));
+    CU_TRY(cudaMemcpy(p.d_idx_bases, idx_bases.data(), sizeof(uint64_t) * idx_bases.size(), cudaMemcpyHostToDevice));
+  }
   p.device = peer_device;
   p.block_stride = stride;
   p.n_blocks = n_blocks;
@@ -1550,7 +1728,7 @@ extern "C" int b200kv_import_peer(b200kv_ctx* ctx, int32_t peer_id, int32_t peer
                                   const b200kv_ipc_desc* descs, int32_t n_descs,
                                   uint64_t peer_block_stride_bytes, uint64_t peer_n_blocks) {
   if (!ctx || !descs || peer_id < 0 || peer_id >= kMaxPeers) return B200KV_EINVAL;
-  if (n_descs != static_cast<int32_t>(ctx->g.planes) || peer_n_blocks == 0 ||
+  if (n_descs != static_cast<int32_t>(n_descs_of(ctx->g)) || peer_n_blocks == 0 ||
       peer_n_blocks * ctx->g.bs > 0x7fffffffull)
     return B200KV_EINVAL;
   DeviceGuard dg(ctx->cfg.device);
@@ -1558,10 +1736,10 @@ extern "C" int b200kv_import_peer(b200kv_ctx* ctx, int32_t peer_id, int32_t peer
   // one cudaIpcOpenMemHandle per distinct allocation
   std::vector<std::pair<std::string, void*>> seen;
   std::vector<void*> opened;
-  std::vector<uint64_t> bases(ctx->g.planes);
+  std::vector<uint64_t> bases(ctx->g.planes), idx_bases(ctx->g.indexed ? ctx->g.L : 0);
   const uint32_t ppl = ctx->g.planes_per_layer;
   for (uint32_t l = 0; l < ctx->g.L; ++l) {
-    for (uint32_t kv = 0; kv < ppl; ++kv) {
+    for (uint32_t kv = 0; kv < n_descs_of(ctx->g) / ctx->g.L; ++kv) {
       const b200kv_ipc_desc& d = descs[kv * ctx->g.L + l];
       const std::string key(reinterpret_cast<const char*>(d.handle), 64);
       void* base = nullptr;
@@ -1574,17 +1752,17 @@ extern "C" int b200kv_import_peer(b200kv_ctx* ctx, int32_t peer_id, int32_t peer
         seen.emplace_back(key, base);
         opened.push_back(base);
       }
-      bases[ppl * l + kv] = reinterpret_cast<uint64_t>(base) + d.offset;
+      (kv < ppl ? bases[ppl * l + kv] : idx_bases[l]) = reinterpret_cast<uint64_t>(base) + d.offset;
     }
   }
   return install_peer(ctx, peer_id, peer_device, bases, peer_block_stride_bytes, peer_n_blocks,
-                      std::move(opened));
+                      std::move(opened), idx_bases);
 }
 
 extern "C" int b200kv_import_peer_ptrs(b200kv_ctx* ctx, int32_t peer_id, int32_t peer_device,
                                        const void* const* k_ptrs, const void* const* v_ptrs,
                                        uint64_t peer_block_stride_bytes, uint64_t peer_n_blocks) {
-  if (!ctx || !k_ptrs || (ctx->g.planes_per_layer == 2) != (v_ptrs != nullptr) || peer_id < 0 ||
+  if (!ctx || !k_ptrs || (ctx->g.planes_per_layer == 2 || ctx->g.indexed) != (v_ptrs != nullptr) || peer_id < 0 ||
       peer_id >= kMaxPeers)
     return B200KV_EINVAL;
   if (peer_n_blocks == 0 || peer_n_blocks * ctx->g.bs > 0x7fffffffull) return B200KV_EINVAL;
@@ -1609,7 +1787,12 @@ extern "C" int b200kv_import_peer_ptrs(b200kv_ctx* ctx, int32_t peer_id, int32_t
       if (!bases[ppl * l + kv] || bases[ppl * l + kv] % 16) return B200KV_EINVAL;
     }
   }
-  return install_peer(ctx, peer_id, peer_device, bases, peer_block_stride_bytes, peer_n_blocks, {});
+  std::vector<uint64_t> idx_bases;   // an engine with indexer planes takes the peer's in v_ptrs
+  for (uint32_t l = 0; ctx->g.indexed && l < ctx->g.L; ++l) {
+    idx_bases.push_back(reinterpret_cast<uint64_t>(v_ptrs[l]));
+    if (!idx_bases.back() || idx_bases.back() % 16) return B200KV_EINVAL;
+  }
+  return install_peer(ctx, peer_id, peer_device, bases, peer_block_stride_bytes, peer_n_blocks, {}, idx_bases);
 }
 
 extern "C" int b200kv_peer_pull_async(b200kv_ctx* ctx, int32_t peer_id, const int64_t* src_slots,
@@ -1664,6 +1847,7 @@ extern "C" int b200kv_peer_pull_async(b200kv_ctx* ctx, int32_t peer_id, const in
   ++ctx->stats.n_pull_ops;
   ctx->stats.n_pulled_tokens += n_tokens;
   ctx->stats.p2p_bytes += static_cast<uint64_t>(n_tokens) * ctx->g.token_bytes * ctx->g.planes;
+  if (ctx->g.indexed) ctx->stats.p2p_bytes += static_cast<uint64_t>(n_tokens) * (ctx->g.idx_vb + ctx->g.idx_sb) * ctx->g.L;
   *ticket = op->id;
   ctx->ops.emplace(op->id, std::move(guard.op));
   guard.armed = false;

@@ -31,6 +31,8 @@
 //   kv_q4_load_kernel      of lanes.
 //   kv_mla_fp8_store_kernel /  FP8 latent records of MLA engines: one warp per (token, plane), a group of
 //   kv_mla_fp8_load_kernel     128 elements is 16 lanes; no shared memory.
+//   kv_indexer_copy_kernel the indexer planes of sparse-attention MLA engines (split [values][scales] tiles),
+//                          verbatim, store / load / pull: TMA bulk pieces, a 4-byte warp copy for unaligned scales.
 //
 // Every kernel takes one KernelArgs, filled by kernel_args() in b200kv_engine.cu.  The seven FP8 / Q4 / MLA FP8
 // kernels are also built per cache element type (bf16, fp16: template argument DT, see Src below).
@@ -1136,6 +1138,79 @@ __global__ void __launch_bounds__(kMlaThreads) kv_mla_fp8_load_kernel(const Kern
       }
     }
   }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Indexer planes of a sparse-attention MLA engine (b200kv_set_indexer; spec: tests/mla_sparse_oracle.py):
+// DeepSeek-V3.2's indexer key cache, one split tile per block ([bs][vb] values, then [bs][sb] scales), copied
+// verbatim between the pages and a chunk's indexer slabs ([C][vb], then [C][sb] per layer), or from a peer's pages.
+// Store, load and pull; launched by launch_op right after the latent kernel of the same runs, on the same stream.
+// KernelArgs describe the indexer planes here:
+//   paged / peer  bases = the L indexer planes, block_stride = their block stride, token_bytes = vb
+//   chunk         slab_bytes = one layer's indexer slab C*(vb+sb), scales_off = where the indexer slabs start
+//   row_bytes     sb
+// A unit is one (run, layer): total_units = n_runs * n_planes.  Each warp takes one unit at a time through its own
+// shared-memory stage of bs*(vb+sb) bytes: lane 0 moves the value piece, and the scale piece when it is 16-byte
+// granular (bulk_piece: every whole block when bs % 4 == 0), with the TMA engine (global -> smem -> global, the
+// stores of one unit overlapping the loads of the next); any other scale piece is copied by the warp, 4 bytes per
+// lane.  A run never crosses a block, so a stage holds any unit.
+// ---------------------------------------------------------------------------------------------
+constexpr int kIdxWarps = 4;
+constexpr uint32_t kIdxBarBytes = 128;   // the warps' mbarriers, ahead of the stages
+
+__device__ __forceinline__ uint32_t idx_stage_bytes(uint32_t bs, uint32_t vb, uint32_t sb) {
+  return (bs * (vb + sb) + 15u) & ~15u;
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(kIdxWarps * 32) kv_indexer_copy_kernel(const KernelArgs p) {
+  extern __shared__ __align__(128) uint8_t smem[];
+  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
+  const uint32_t bs = p.paged.block_tokens, vb = p.paged.token_bytes, sb = p.row_bytes;
+  uint64_t* bar = reinterpret_cast<uint64_t*>(smem) + warp;
+  uint8_t* stage = smem + kIdxBarBytes + static_cast<size_t>(warp) * idx_stage_bytes(bs, vb, sb);
+  uint8_t* stage_s = stage + static_cast<size_t>(bs) * vb;
+  if (lane == 0) {
+    mbar_init(bar, 1);
+    fence_mbar_init();
+  }
+  __syncwarp();
+  const SplitTile tile{bs, p.chunk.chunk_tokens, vb, sb, MODE == kPull ? p.peer.block_stride : p.paged.block_stride,
+                       p.paged.block_stride};
+  uint32_t phase = 0;
+  for (uint32_t u = blockIdx.x * kIdxWarps + warp; u < p.total_units; u += gridDim.x * kIdxWarps, phase ^= 1u) {
+    const uint32_t plane = p.plane_begin + u % p.n_planes;
+    const Run run = p.runs[u / p.n_planes];
+    SplitPiece v, s;
+    split_run_pieces(tile, MODE, run, &v, &s);
+    // the offsets' bases: pages at slot run.a, and the chunk slab (store / load) or local pages (pull) at run.b
+    const uint64_t page_a = __ldg((MODE == kPull ? p.peer.bases : p.paged.bases) + plane);
+    const uint64_t side_b = MODE == kPull ? __ldg(p.paged.bases + plane)
+                                          : __ldg(p.chunk.chunk_addrs + chunk_pos(p.chunk, static_cast<uint32_t>(run.b)).c) +
+                                                p.chunk.scales_off + static_cast<uint64_t>(plane) * p.chunk.slab_bytes;
+    const uint64_t src_base = MODE == kLoad ? side_b : page_a, dst_base = MODE == kLoad ? page_a : side_b;
+    v.src += src_base; v.dst += dst_base;
+    s.src += src_base; s.dst += dst_base;
+    const bool s_bulk = bulk_piece(s);
+    if (lane == 0) {
+      bulk_wait_read<0>();   // the previous unit's stores have read the stage
+      mbar_arrive_expect_tx(bar, v.bytes + (s_bulk ? s.bytes : 0u));
+      bulk_g2s(stage, reinterpret_cast<const void*>(v.src), v.bytes, bar);
+      if (s_bulk) bulk_g2s(stage_s, reinterpret_cast<const void*>(s.src), s.bytes, bar);
+    }
+    if (!s_bulk) {
+      const uint32_t* src = reinterpret_cast<const uint32_t*>(s.src);
+      uint32_t* dst = reinterpret_cast<uint32_t*>(s.dst);
+      for (uint32_t i = lane; i < s.bytes / 4; i += 32) dst[i] = __ldg(src + i);
+    }
+    if (lane == 0) {
+      mbar_wait(bar, phase);
+      bulk_s2g(reinterpret_cast<void*>(v.dst), stage, v.bytes);
+      if (s_bulk) bulk_s2g(reinterpret_cast<void*>(s.dst), stage_s, s.bytes);
+      bulk_commit();
+    }
+  }
+  if (lane == 0) bulk_wait_all<0>();   // every store has landed before the grid is considered complete
 }
 
 }  // namespace b200kv

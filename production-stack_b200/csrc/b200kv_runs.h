@@ -164,6 +164,67 @@ inline bool whole_block_chunks(const OpTable& t, int32_t bs, int32_t C) {
   return true;
 }
 
+// ---- split tiles: the indexer key cache of DeepSeek-V3.2's sparse attention (b200kv_set_indexer) -----------------
+// vLLM's indexer_k_quant_and_cache writes a block of bs tokens as [bs][vb] values followed by [bs][sb] scales (one
+// fp32 per token), so a tile is not token-major.  A chunk's indexer slab of one layer mirrors the tile: [C][vb]
+// values, then [C][sb] scales.  A run (consecutive tokens inside one block and one chunk) is therefore two
+// contiguous pieces on each side, n*vb value bytes and n*sb scale bytes.  These helpers give the pieces of a run as
+// offsets: relative to the plane's block 0 on a page side, to the layer's indexer slab of the run's chunk on the
+// chunk side.  kv_indexer_copy_kernel calls the same code on the device.
+#if defined(__CUDACC__)
+#define B200KV_HD __host__ __device__ __forceinline__
+#else
+#define B200KV_HD inline
+#endif
+
+struct SplitTile {
+  uint32_t bs, C, vb, sb;
+  uint64_t a_stride;   // block stride of the pages at slot run.a: the local pages of a store / load, a pull's source
+  uint64_t b_stride;   // a pull: block stride of the destination pages at slot run.b
+};
+
+struct SplitPiece {
+  uint64_t src, dst;
+  uint32_t bytes;
+};
+
+// value and scale offsets of slot `slot` inside pages of block stride `stride`
+B200KV_HD void split_page_offsets(const SplitTile& t, uint64_t stride, uint32_t slot, uint64_t* v, uint64_t* s) {
+  const uint32_t blk = slot / t.bs, off = slot - blk * t.bs;
+  const uint64_t b = static_cast<uint64_t>(blk) * stride;
+  *v = b + static_cast<uint64_t>(off) * t.vb;
+  *s = b + static_cast<uint64_t>(t.bs) * t.vb + static_cast<uint64_t>(off) * t.sb;
+}
+
+// value and scale offsets of op-relative token `tok` inside its chunk's slab
+B200KV_HD void split_chunk_offsets(const SplitTile& t, uint32_t tok, uint64_t* v, uint64_t* s) {
+  const uint32_t ct = tok % t.C;
+  *v = static_cast<uint64_t>(ct) * t.vb;
+  *s = static_cast<uint64_t>(t.C) * t.vb + static_cast<uint64_t>(ct) * t.sb;
+}
+
+// The value piece and the scale piece of run r.  mode: 0 = store (pages at slot r.a -> chunk at op token r.b),
+// 1 = load (the reverse), 2 = pull (source pages at slot r.a -> destination pages at slot r.b).
+B200KV_HD void split_run_pieces(const SplitTile& t, int mode, const Run& r, SplitPiece* val, SplitPiece* sc) {
+  uint64_t av, as, bv, bsc;   // side a: pages at slot r.a; side b: the chunk (or the destination pages) at r.b
+  split_page_offsets(t, t.a_stride, static_cast<uint32_t>(r.a), &av, &as);
+  if (mode == 2) split_page_offsets(t, t.b_stride, static_cast<uint32_t>(r.b), &bv, &bsc);
+  else split_chunk_offsets(t, static_cast<uint32_t>(r.b), &bv, &bsc);
+  const uint32_t nv = static_cast<uint32_t>(r.n) * t.vb, ns = static_cast<uint32_t>(r.n) * t.sb;
+  if (mode == 1) {   // chunk -> pages
+    *val = {bv, av, nv};
+    *sc = {bsc, as, ns};
+  } else {
+    *val = {av, bv, nv};
+    *sc = {as, bsc, ns};
+  }
+}
+
+// A piece may go through the TMA engine when both ends and its size are 16-byte multiples (the bases of both sides
+// are 16-byte aligned, so this holds for the offsets exactly when it holds for the addresses).  Value pieces always
+// qualify (vb % 16 == 0); scale pieces do for whole blocks when bs % 4 == 0 and C % 4 == 0.
+B200KV_HD bool bulk_piece(const SplitPiece& p) { return ((p.src | p.dst | p.bytes) & 15u) == 0; }
+
 // Byte layout of a table as the kernels read it: the runs, the chunk addresses, then full_off (the FP8
 // store kernels' per-chunk run offsets), each rounded up to 16 bytes.  A table over kTableBytes is refused.
 constexpr size_t kTableBytes = 1u << 20;
