@@ -262,9 +262,8 @@ int b200kv_set_cache_dtype(b200kv_ctx* ctx, int32_t dtype);
  * multiple of 16).  value_bytes % 16 == 0, scale_bytes % 4 == 0.  Legal between b200kv_engine_create and
  * b200kv_register_kv (and before b200kv_tier_create): -EBUSY after; -EINVAL on an engine that is not MLA.  The
  * staging ring is re-cut to the larger chunk; a pool whose slots are smaller than it gives -EINVAL.  From then on
- * b200kv_register_kv and b200kv_import_peer_ptrs take the indexer planes in v_ptrs, b200kv_export_ipc /
- * b200kv_import_peer take 2*L descriptors (latent planes, then indexer planes), and a peer's indexer planes are
- * taken to have this engine's indexer block stride.                                           */
+ * the indexer planes are the engine's second kind of plane ("Planes and descriptors" at b200kv_register_kv), and a
+ * peer's indexer planes are taken to have this engine's indexer block stride.                 */
 int b200kv_set_indexer(b200kv_ctx* ctx, int32_t value_bytes, int32_t scale_bytes, uint64_t block_stride_bytes);
 /* What the engine did about host-page placement when it pinned the pool (numa_policy above), as text
  * for logs and bench output, e.g. "mbind preferred node 1".                                  */
@@ -277,12 +276,19 @@ int64_t b200kv_engine_chunk_bytes(const b200kv_engine_config* cfg);
  * L * C * 656 (FP8 records).  -EINVAL for a geometry that is not MLA.                         */
 int64_t b200kv_engine_chunk_bytes_indexed(const b200kv_engine_config* cfg, int32_t value_bytes, int32_t scale_bytes);
 
-/* register_kv_caches (KVConnectorBase_V1, vllm/.../v1/base.py:251): device base address of
- * block 0 of each layer's K and V planes, NHD within a block ([block_tokens][H][D]).
+/* Planes and descriptors.  An engine has one or two kinds of plane per layer, passed as k_ptrs[l] and v_ptrs[l]
+ * (device address of block 0 of layer l's plane, non-null and 16-byte aligned):
+ *   B200KV_LAYOUT_NHD / _HND      k_ptrs: K planes    v_ptrs: V planes
+ *   B200KV_LAYOUT_MLA             k_ptrs: latent      v_ptrs: NULL
+ *   MLA after b200kv_set_indexer  k_ptrs: latent      v_ptrs: indexer planes
+ * Anything else gives -EINVAL.  IPC descriptors follow the same order, kind-major: descriptor i is plane
+ * (i / L, i % L), so there are 2*L of them with two kinds (k_ptrs' planes first) and L with one.
+ *
+ * register_kv_caches (KVConnectorBase_V1, vllm/.../v1/base.py:251): the engine's planes as above, NHD within a
+ * block ([block_tokens][H][D]).
  * FlashAttention (2,NB,bs,H,D): v = k + NB*tile; FlashInfer (NB,2,bs,H,D): v = k + tile,
  * block_stride = 2*tile; cross-layer (NB,L,2,bs,H,D): block_stride = 2*L*tile.
- * B200KV_LAYOUT_MLA: k_ptrs are the layers' latent planes and v_ptrs must be NULL, or the layers' indexer
- * planes after b200kv_set_indexer.                                                           */
+ * A refused call leaves the registration as it was.                                          */
 int b200kv_register_kv(b200kv_ctx* ctx, const void* const* k_ptrs, const void* const* v_ptrs);
 
 /* lmcache_engine.store (vllm_v1_adapter.py:1115-1123).  Tokens [0,n_tokens) start on a
@@ -359,16 +365,16 @@ typedef struct b200kv_ipc_desc {
   uint64_t alloc_bytes; /* size of the allocation (informational)                            */
 } b200kv_ipc_desc;
 
-/* Export 2*L descriptors (K planes then V planes) of the registered cache; L (one per layer's
- * latent plane) for B200KV_LAYOUT_MLA, 2*L (latent planes then indexer planes) after
- * b200kv_set_indexer.  import_peer takes as many; import_peer_ptrs takes v_ptrs NULL for MLA,
- * and the indexer planes in v_ptrs after b200kv_set_indexer.                               */
+/* Export the descriptors of the registered cache, one per plane in the order given at
+ * b200kv_register_kv; n_descs must be their count.  import_peer takes as many.             */
 int b200kv_export_ipc(b200kv_ctx* ctx, b200kv_ipc_desc* descs_out, int32_t n_descs);
-/* Map a peer replica's cache (same model geometry).  `peer_id` is caller-chosen (0..63).   */
+/* Map a peer replica's cache (same model geometry).  `peer_id` is caller-chosen (0..63).  An
+ * import that is refused or fails installs nothing and keeps no mapping open (both imports). */
 int b200kv_import_peer(b200kv_ctx* ctx, int32_t peer_id, int32_t peer_device,
                        const b200kv_ipc_desc* descs, int32_t n_descs,
                        uint64_t peer_block_stride_bytes, uint64_t peer_n_blocks);
-/* Same-process variant (tests, single-process multi-GPU): raw peer device pointers.        */
+/* Same-process variant (tests, single-process multi-GPU): raw peer device pointers, k_ptrs and
+ * v_ptrs as at b200kv_register_kv.                                                          */
 int b200kv_import_peer_ptrs(b200kv_ctx* ctx, int32_t peer_id, int32_t peer_device,
                             const void* const* k_ptrs, const void* const* v_ptrs,
                             uint64_t peer_block_stride_bytes, uint64_t peer_n_blocks);

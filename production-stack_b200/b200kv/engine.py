@@ -128,6 +128,11 @@ class KVGeometry:
         return self.n_layers * (1 if self.mla else 2)
 
     @property
+    def n_descs(self) -> int:
+        """IPC descriptors of the engine's cache (b200kv_export_ipc): one per paged plane and per indexer plane."""
+        return self.planes + (self.n_layers if self.indexed else 0)
+
+    @property
     def stride(self) -> int:
         return self.block_stride_bytes or self.block_tokens * self.token_bytes
 
@@ -442,20 +447,19 @@ class KVEngine:
         """kv_caches: list (or dict) of per-layer torch tensors on this device.  With indexer planes, the latent and
         indexer caches of every layer (split_indexer_caches tells them apart)."""
         tensors = list(kv_caches.values()) if isinstance(kv_caches, dict) else list(kv_caches)
-        idx_ptrs = None
+        # v_ptrs: the V planes, the indexer planes, or None (plain MLA); include/b200kv.h, "Planes and descriptors"
+        lat, k_ptrs, v_ptrs = tensors, [], (None if self.geom.mla else [])
         if self.geom.indexed:
             lat, idx = split_indexer_caches(kv_caches, self.geom.idx_token_bytes)
             if not idx:
                 raise ValueError("the engine has indexer planes but no indexer cache was given")
-            idx_ptrs = []
+            v_ptrs = []
             for t in idx:
                 ptr, stride, nb = indexer_layout_of(t, self.geom.block_tokens, self.geom.idx_token_bytes)
                 if stride != self.geom.idx_stride or nb < self.geom.n_blocks:
                     raise ValueError("indexer cache tensor does not match the engine geometry")
-                idx_ptrs.append(ptr)
-            tensors_all, tensors = tensors, lat
-        ks, vs = [], []
-        for t in tensors:
+                v_ptrs.append(ptr)
+        for t in lat:
             k, v, stride, nb, h, d, tl = paged_layout_of(t, self.geom.block_tokens, layout)
             if stride != self.geom.stride or h != self.geom.n_kv_heads or d != self.geom.head_dim \
                     or nb < self.geom.n_blocks or t.element_size() != self.geom.elem_bytes \
@@ -466,10 +470,11 @@ class KVEngine:
                 # and loaded as wrong values without any error
                 raise ValueError(f"KV cache dtype {t.dtype} does not match the engine's cache dtype "
                                  f"({'float16' if self.geom.fp16 else 'bfloat16'})")
-            ks.append(k)
-            vs.append(v)
-        self._kv_refs = tensors if idx_ptrs is None else tensors_all  # keep the storage alive
-        self.register_kv_ptrs(ks, idx_ptrs if self.geom.mla else vs)
+            k_ptrs.append(k)
+            if not self.geom.mla:
+                v_ptrs.append(v)
+        self._kv_refs = tensors   # keep the storage of every registered tensor alive
+        self.register_kv_ptrs(k_ptrs, v_ptrs)
 
     # ---- LMCache-shaped data path ---------------------------------------------------------
     def _keys(self, tokens) -> np.ndarray:
@@ -640,14 +645,14 @@ class KVEngine:
                                           _stream_ptr(stream)), "b200kv_scatter_chunks")
 
     def export_ipc(self) -> bytes:
-        n = self.geom.planes + (self.geom.n_layers if self.geom.indexed else 0)
+        n = self.geom.n_descs
         arr = (_lib.IpcDesc * n)()
         check(lib().b200kv_export_ipc(self._h, arr, n), "b200kv_export_ipc")
         return bytes(arr)
 
     def import_peer(self, peer_id: int, peer_device: int, descs: bytes,
                     peer_block_stride: int | None = None, peer_n_blocks: int | None = None):
-        n = self.geom.planes + (self.geom.n_layers if self.geom.indexed else 0)
+        n = self.geom.n_descs
         arr = (_lib.IpcDesc * n).from_buffer_copy(descs)
         check(lib().b200kv_import_peer(self._h, peer_id, peer_device, arr, n,
                                         peer_block_stride or self.geom.stride,

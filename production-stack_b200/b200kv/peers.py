@@ -18,7 +18,8 @@ def all_gather_bytes(payload: bytes, group=None) -> list[bytes]:
 
 
 def exchange_kv_descriptors(engine, group=None) -> list[bytes]:
-    """Every rank exports its 2*L descriptors (b200kv_export_ipc); returns them indexed by rank."""
+    """Every rank exports its descriptors (b200kv_export_ipc, KVGeometry.n_descs of them); returns them indexed by
+    rank."""
     return all_gather_bytes(engine.export_ipc(), group)
 
 

@@ -132,8 +132,7 @@ struct OpGuard {
 struct Peer {
   bool valid = false;
   int device = -1;
-  uint64_t* d_bases = nullptr;
-  uint64_t* d_idx_bases = nullptr;   // indexer planes (engines with b200kv_set_indexer); same block stride as ours
+  uint64_t* d_bases = nullptr;       // the peer's base table, slots as ours (base_slot); indexer planes have our stride
   uint64_t block_stride = 0;
   uint64_t n_blocks = 0;
   std::vector<void*> opened;  // cudaIpcOpenMemHandle mappings to close
@@ -142,6 +141,7 @@ struct Peer {
 struct Geometry {
   uint32_t L, H, D, elem, bs, C, planes;
   uint32_t planes_per_layer;  // 2 (K, V), or 1 (MLA latent)
+  uint32_t n_bases;       // base-table slots, one per IPC descriptor: the planes, then L indexer planes (indexed)
   uint32_t token_bytes;   // H*D*elem
   uint64_t slab_bytes;    // C*token_bytes (RAW) or C*H*D (FP8)
   uint64_t chunk_bytes;
@@ -179,6 +179,7 @@ int make_geometry(const b200kv_engine_config* c, Geometry* g) {
   if (g->mla && g->H != 1) return B200KV_EINVAL;  // the latent is per token, not per head
   g->planes_per_layer = g->mla ? 1u : 2u;
   g->planes = g->planes_per_layer * g->L;
+  g->n_bases = g->planes;
   g->token_bytes = g->H * g->D * g->elem;
   g->row_bytes = g->D * g->elem;
   g->dtype = B200KV_DTYPE_BF16;
@@ -236,12 +237,34 @@ int add_indexer(Geometry* g, int64_t value_bytes, int64_t scale_bytes, uint64_t 
   const uint64_t slab = static_cast<uint64_t>(g->C) * static_cast<uint64_t>(value_bytes + scale_bytes);
   if (slab % 16) return B200KV_EINVAL;   // every slab starts on a 16-byte boundary (bulk copies)
   g->indexed = true;
+  g->n_bases = g->planes + g->L;
   g->idx_vb = static_cast<uint32_t>(value_bytes);
   g->idx_sb = static_cast<uint32_t>(scale_bytes);
   g->idx_stride = block_stride;
   g->idx_off = g->slab_bytes * g->planes;
   g->idx_slab = slab;
   g->chunk_bytes = (g->idx_off + g->idx_slab * g->L + 255) / 256 * 256;
+  return B200KV_OK;
+}
+
+// Base-table slot of plane (kind, l) as callers order planes (b200kv.h, "Planes and descriptors"; descriptor i is
+// (i / L, i % L)): kernels index ppl*l + kind, and indexer planes follow at planes + l.  The only order conversion.
+uint32_t base_slot(const Geometry& g, uint32_t kind, uint32_t l) {
+  return kind < g.planes_per_layer ? g.planes_per_layer * l + kind : g.planes + l;
+}
+
+// (k_ptrs, v_ptrs) -> the full base table.  v_ptrs is given exactly when the engine has a second kind of plane, and
+// every pointer is non-null and 16-byte aligned; otherwise -EINVAL.
+int plane_bases(const Geometry& g, const void* const* k_ptrs, const void* const* v_ptrs, std::vector<uint64_t>* out) {
+  const uint32_t kinds = g.n_bases / g.L;
+  if (!k_ptrs || (kinds == 2) != (v_ptrs != nullptr)) return B200KV_EINVAL;
+  out->assign(g.n_bases, 0);
+  for (uint32_t kind = 0; kind < kinds; ++kind)
+    for (uint32_t l = 0; l < g.L; ++l) {
+      const uint64_t p = reinterpret_cast<uint64_t>((kind ? v_ptrs : k_ptrs)[l]);
+      if (!p || p % 16) return B200KV_EINVAL;
+      (*out)[base_slot(g, kind, l)] = p;
+    }
   return B200KV_OK;
 }
 
@@ -269,10 +292,9 @@ struct b200kv_ctx {
 
   cudaStream_t s_gather = nullptr, s_d2h = nullptr, s_h2d = nullptr, s_scatter = nullptr;
   cudaEvent_t fence = nullptr;          // stream_wait's event
-  uint64_t* d_bases = nullptr;
-  uint64_t* d_idx_bases = nullptr;      // [L] indexer planes (g.indexed)
+  uint64_t* d_bases = nullptr;          // the base table, g.n_bases slots (base_slot)
   bool kv_registered = false;
-  std::vector<const void*> h_k, h_v;
+  std::vector<uint64_t> h_bases;        // the registered base table on the host (export_ipc)
 
   uint8_t* d_staging = nullptr;
   std::vector<StageSlot> stage;
@@ -588,11 +610,11 @@ int launch_indexer(b200kv_ctx* ctx, CopyMode mode, const TableView& tv, size_t f
                    uint32_t pb, uint32_t np, const Peer* peer) {
   const Geometry& g = ctx->g;
   KernelArgs a = kernel_args(ctx, tv, f0, pb, np, peer);
-  a.paged.bases = ctx->d_idx_bases;
+  a.paged.bases = ctx->d_bases + g.planes;
   a.paged.block_stride = g.idx_stride;
   a.paged.token_bytes = g.idx_vb;
   a.peer = a.paged;
-  if (peer) a.peer.bases = peer->d_idx_bases;
+  if (peer) a.peer.bases = peer->d_bases + g.planes;
   a.chunk.slab_bytes = g.idx_slab;
   a.chunk.scales_off = g.idx_off;
   a.chunk.token_bytes = g.idx_vb;
@@ -966,7 +988,8 @@ static int engine_create_impl(const b200kv_engine_config* cfg, b200kv_pool* pool
     CU_TRY(cudaFuncSetAttribute(kv_fp8_store_kernel<kFp16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   }
 
-  CU_TRY(cudaMalloc(&ctx->d_bases, sizeof(uint64_t) * g.planes));
+  // 2*L slots, the most any geometry uses, so b200kv_set_indexer has nothing to allocate
+  CU_TRY(cudaMalloc(&ctx->d_bases, sizeof(uint64_t) * 2 * g.L));
 
   rc = make_staging(ctx, g.chunk_bytes);
   if (rc) return rc;
@@ -1022,7 +1045,6 @@ extern "C" int b200kv_engine_destroy(b200kv_ctx* ctx) {
     if (!p.valid) continue;
     for (void* m : p.opened) cudaIpcCloseMemHandle(m);
     cudaFree(p.d_bases);
-    if (p.d_idx_bases) cudaFree(p.d_idx_bases);
   }
   for (auto& t : ctx->tables) {
     if (t.host) cudaFreeHost(t.host);
@@ -1041,7 +1063,6 @@ extern "C" int b200kv_engine_destroy(b200kv_ctx* ctx) {
   for (void* m : ctx->tier_imports) cudaIpcCloseMemHandle(m);
   if (ctx->tier_base) cudaFree(ctx->tier_base);
   if (ctx->d_bases) cudaFree(ctx->d_bases);
-  if (ctx->d_idx_bases) cudaFree(ctx->d_idx_bases);
   if (ctx->d_tmaps) cudaFree(ctx->d_tmaps);
   if (ctx->fence) cudaEventDestroy(ctx->fence);
   for (cudaStream_t s : {ctx->s_gather, ctx->s_d2h, ctx->s_h2d, ctx->s_scatter})
@@ -1133,7 +1154,6 @@ extern "C" int b200kv_set_indexer(b200kv_ctx* ctx, int32_t value_bytes, int32_t 
   typedef void (*IndexerKernel)(KernelArgs);
   for (IndexerKernel k : {kv_indexer_copy_kernel<kStore>, kv_indexer_copy_kernel<kLoad>, kv_indexer_copy_kernel<kPull>})
     CU_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(indexer_smem_bytes(g))));
-  if (!ctx->d_idx_bases) CU_TRY(cudaMalloc(&ctx->d_idx_bases, sizeof(uint64_t) * g.L));
   rc = make_staging(ctx, g.chunk_bytes);   // the engine keeps its geometry and ring if this fails
   if (rc) return rc;
   ctx->g = g;
@@ -1142,31 +1162,15 @@ extern "C" int b200kv_set_indexer(b200kv_ctx* ctx, int32_t value_bytes, int32_t 
 
 extern "C" int b200kv_register_kv(b200kv_ctx* ctx, const void* const* k_ptrs,
                                   const void* const* v_ptrs) {
-  const uint32_t ppl = ctx ? ctx->g.planes_per_layer : 0;
-  // MLA: v_ptrs NULL, or the indexer planes on an engine with b200kv_set_indexer
-  if (!ctx || !k_ptrs || (ppl == 2 || ctx->g.indexed) != (v_ptrs != nullptr)) return B200KV_EINVAL;
+  if (!ctx) return B200KV_EINVAL;
   DeviceGuard dg(ctx->cfg.device);
   std::lock_guard<std::mutex> lk(ctx->mu);
-  std::vector<uint64_t> h(ctx->g.planes);
-  ctx->h_k.assign(k_ptrs, k_ptrs + ctx->g.L);
-  if (v_ptrs) ctx->h_v.assign(v_ptrs, v_ptrs + ctx->g.L);
-  for (uint32_t l = 0; l < ctx->g.L; ++l) {
-    for (uint32_t kv = 0; kv < ppl; ++kv) {
-      const uint64_t p = reinterpret_cast<uint64_t>(kv ? v_ptrs[l] : k_ptrs[l]);
-      if (!p || p % 16) return B200KV_EINVAL;
-      h[ppl * l + kv] = p;
-    }
-  }
-  if (ctx->g.indexed) {
-    std::vector<uint64_t> hi(ctx->g.L);
-    for (uint32_t l = 0; l < ctx->g.L; ++l) {
-      hi[l] = reinterpret_cast<uint64_t>(v_ptrs[l]);
-      if (!hi[l] || hi[l] % 16) return B200KV_EINVAL;
-    }
-    CU_TRY(cudaMemcpy(ctx->d_idx_bases, hi.data(), sizeof(uint64_t) * hi.size(), cudaMemcpyHostToDevice));
-  }
+  std::vector<uint64_t> h;
+  const int rc = plane_bases(ctx->g, k_ptrs, v_ptrs, &h);
+  if (rc) return rc;
   CU_TRY(cudaMemcpy(ctx->d_bases, h.data(), sizeof(uint64_t) * h.size(), cudaMemcpyHostToDevice));
-  build_tensor_maps(ctx, h);
+  ctx->h_bases = std::move(h);
+  build_tensor_maps(ctx, ctx->h_bases);
   if (env_int("B200KV_VERBOSE", 0)) std::fprintf(stderr, "b200kv: tensor maps: %s\n", ctx->tmap_status.c_str());
   ctx->kv_registered = true;
   return B200KV_OK;
@@ -1673,12 +1677,10 @@ extern "C" int b200kv_wait_all(b200kv_ctx* ctx) {
 // ------------------------------------------------------------------------------------------------
 // peers
 // ------------------------------------------------------------------------------------------------
-// IPC descriptors of an engine's planes: K and V (2L), latent (L), or latent and indexer (2L) planes
-static uint32_t n_descs_of(const Geometry& g) { return g.planes + (g.indexed ? g.L : 0u); }
-
 extern "C" int b200kv_export_ipc(b200kv_ctx* ctx, b200kv_ipc_desc* descs_out, int32_t n_descs) {
   if (!ctx || !descs_out) return B200KV_EINVAL;
-  if (!ctx->kv_registered || n_descs != static_cast<int32_t>(n_descs_of(ctx->g))) return B200KV_EINVAL;
+  const Geometry& g = ctx->g;
+  if (!ctx->kv_registered || n_descs != static_cast<int32_t>(g.n_bases)) return B200KV_EINVAL;
   DeviceGuard dg(ctx->cfg.device);
   typedef CUresult (*GetRange)(CUdeviceptr*, size_t*, CUdeviceptr);
   void* fn = nullptr;
@@ -1686,41 +1688,42 @@ extern "C" int b200kv_export_ipc(b200kv_ctx* ctx, b200kv_ipc_desc* descs_out, in
   CU_TRY(cudaGetDriverEntryPoint("cuMemGetAddressRange", &fn, cudaEnableDefault, &qr));
   if (!fn || qr != cudaDriverEntryPointSuccess) return B200KV_ENODEV;
   GetRange get_range = reinterpret_cast<GetRange>(fn);
-  for (uint32_t l = 0; l < ctx->g.L; ++l) {
-    for (uint32_t kv = 0; kv < n_descs_of(ctx->g) / ctx->g.L; ++kv) {
-      const void* p = kv ? ctx->h_v[l] : ctx->h_k[l];
-      CUdeviceptr base = 0;
-      size_t size = 0;
-      if (get_range(&base, &size, reinterpret_cast<CUdeviceptr>(p)) != CUDA_SUCCESS) return B200KV_ENODEV;
-      b200kv_ipc_desc& d = descs_out[kv * ctx->g.L + l];  // K planes then V planes (MLA: latent, then indexer planes)
-      std::memset(&d, 0, sizeof(d));
-      cudaIpcMemHandle_t h;
-      CU_TRY(cudaIpcGetMemHandle(&h, reinterpret_cast<void*>(base)));
-      static_assert(sizeof(h) == 64, "cudaIpcMemHandle_t is 64 bytes");
-      std::memcpy(d.handle, &h, 64);
-      d.offset = reinterpret_cast<uint64_t>(p) - static_cast<uint64_t>(base);
-      d.alloc_bytes = size;
-    }
+  for (uint32_t i = 0; i < g.n_bases; ++i) {
+    const uint64_t p = ctx->h_bases[base_slot(g, i / g.L, i % g.L)];
+    CUdeviceptr base = 0;
+    size_t size = 0;
+    if (get_range(&base, &size, static_cast<CUdeviceptr>(p)) != CUDA_SUCCESS) return B200KV_ENODEV;
+    b200kv_ipc_desc& d = descs_out[i];
+    std::memset(&d, 0, sizeof(d));
+    cudaIpcMemHandle_t h;
+    CU_TRY(cudaIpcGetMemHandle(&h, reinterpret_cast<void*>(base)));
+    static_assert(sizeof(h) == 64, "cudaIpcMemHandle_t is 64 bytes");
+    std::memcpy(d.handle, &h, 64);
+    d.offset = p - static_cast<uint64_t>(base);
+    d.alloc_bytes = size;
   }
   return B200KV_OK;
 }
 
-static int install_peer(b200kv_ctx* ctx, int32_t peer_id, int32_t peer_device,
-                        const std::vector<uint64_t>& bases, uint64_t stride, uint64_t n_blocks,
-                        std::vector<void*>&& opened, const std::vector<uint64_t>& idx_bases = {}) {
-  Peer& p = ctx->peers[peer_id];
-  if (p.valid) return B200KV_EEXIST;
+// Installs a peer whole or not at all: ctx->peers[peer_id] is written only once its base table is on the device.
+// It then owns `opened`; on failure nothing of the peer is left, and the caller still owns `opened`.
+static int install_peer(b200kv_ctx* ctx, int32_t peer_id, int32_t peer_device, const std::vector<uint64_t>& bases,
+                        uint64_t stride, uint64_t n_blocks, std::vector<void*>* opened) {
+  if (ctx->peers[peer_id].valid) return B200KV_EEXIST;
+  Peer p;
   CU_TRY(cudaMalloc(&p.d_bases, sizeof(uint64_t) * bases.size()));
-  CU_TRY(cudaMemcpy(p.d_bases, bases.data(), sizeof(uint64_t) * bases.size(), cudaMemcpyHostToDevice));
-  if (!idx_bases.empty()) {
-    CU_TRY(cudaMalloc(&p.d_idx_bases, sizeof(uint64_t) * idx_bases.size()));
-    CU_TRY(cudaMemcpy(p.d_idx_bases, idx_bases.data(), sizeof(uint64_t) * idx_bases.size(), cudaMemcpyHostToDevice));
+  const cudaError_t e = cudaMemcpy(p.d_bases, bases.data(), sizeof(uint64_t) * bases.size(), cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {
+    cudaFree(p.d_bases);
+    set_err("cudaMemcpy(peer bases)", e, __LINE__);
+    return B200KV_ENODEV;
   }
   p.device = peer_device;
   p.block_stride = stride;
   p.n_blocks = n_blocks;
-  p.opened = std::move(opened);
+  p.opened = std::move(*opened);
   p.valid = true;
+  ctx->peers[peer_id] = std::move(p);
   return B200KV_OK;
 }
 
@@ -1728,46 +1731,52 @@ extern "C" int b200kv_import_peer(b200kv_ctx* ctx, int32_t peer_id, int32_t peer
                                   const b200kv_ipc_desc* descs, int32_t n_descs,
                                   uint64_t peer_block_stride_bytes, uint64_t peer_n_blocks) {
   if (!ctx || !descs || peer_id < 0 || peer_id >= kMaxPeers) return B200KV_EINVAL;
-  if (n_descs != static_cast<int32_t>(n_descs_of(ctx->g)) || peer_n_blocks == 0 ||
-      peer_n_blocks * ctx->g.bs > 0x7fffffffull)
+  const Geometry& g = ctx->g;
+  if (n_descs != static_cast<int32_t>(g.n_bases) || peer_n_blocks == 0 || peer_n_blocks * g.bs > 0x7fffffffull)
     return B200KV_EINVAL;
   DeviceGuard dg(ctx->cfg.device);
   std::lock_guard<std::mutex> lk(ctx->mu);
   // one cudaIpcOpenMemHandle per distinct allocation
   std::vector<std::pair<std::string, void*>> seen;
   std::vector<void*> opened;
-  std::vector<uint64_t> bases(ctx->g.planes), idx_bases(ctx->g.indexed ? ctx->g.L : 0);
-  const uint32_t ppl = ctx->g.planes_per_layer;
-  for (uint32_t l = 0; l < ctx->g.L; ++l) {
-    for (uint32_t kv = 0; kv < n_descs_of(ctx->g) / ctx->g.L; ++kv) {
-      const b200kv_ipc_desc& d = descs[kv * ctx->g.L + l];
-      const std::string key(reinterpret_cast<const char*>(d.handle), 64);
-      void* base = nullptr;
-      for (auto& s : seen)
-        if (s.first == key) base = s.second;
-      if (!base) {
-        cudaIpcMemHandle_t h;
-        std::memcpy(&h, d.handle, 64);
-        CU_TRY(cudaIpcOpenMemHandle(&base, h, cudaIpcMemLazyEnablePeerAccess));
-        seen.emplace_back(key, base);
-        opened.push_back(base);
+  std::vector<uint64_t> bases(g.n_bases);
+  int rc = B200KV_OK;
+  for (uint32_t i = 0; i < g.n_bases; ++i) {
+    const b200kv_ipc_desc& d = descs[i];
+    const std::string key(reinterpret_cast<const char*>(d.handle), 64);
+    void* base = nullptr;
+    for (auto& s : seen)
+      if (s.first == key) base = s.second;
+    if (!base) {
+      cudaIpcMemHandle_t h;
+      std::memcpy(&h, d.handle, 64);
+      const cudaError_t e = cudaIpcOpenMemHandle(&base, h, cudaIpcMemLazyEnablePeerAccess);
+      if (e != cudaSuccess) {
+        set_err("cudaIpcOpenMemHandle", e, __LINE__);
+        rc = B200KV_ENODEV;
+        break;
       }
-      (kv < ppl ? bases[ppl * l + kv] : idx_bases[l]) = reinterpret_cast<uint64_t>(base) + d.offset;
+      seen.emplace_back(key, base);
+      opened.push_back(base);
     }
+    bases[base_slot(g, i / g.L, i % g.L)] = reinterpret_cast<uint64_t>(base) + d.offset;
   }
-  return install_peer(ctx, peer_id, peer_device, bases, peer_block_stride_bytes, peer_n_blocks,
-                      std::move(opened), idx_bases);
+  if (rc == B200KV_OK) rc = install_peer(ctx, peer_id, peer_device, bases, peer_block_stride_bytes, peer_n_blocks, &opened);
+  if (rc)   // the mappings this call opened; install_peer took none of them
+    for (void* m : opened) cudaIpcCloseMemHandle(m);
+  return rc;
 }
 
 extern "C" int b200kv_import_peer_ptrs(b200kv_ctx* ctx, int32_t peer_id, int32_t peer_device,
                                        const void* const* k_ptrs, const void* const* v_ptrs,
                                        uint64_t peer_block_stride_bytes, uint64_t peer_n_blocks) {
-  if (!ctx || !k_ptrs || (ctx->g.planes_per_layer == 2 || ctx->g.indexed) != (v_ptrs != nullptr) || peer_id < 0 ||
-      peer_id >= kMaxPeers)
-    return B200KV_EINVAL;
+  if (!ctx || peer_id < 0 || peer_id >= kMaxPeers) return B200KV_EINVAL;
   if (peer_n_blocks == 0 || peer_n_blocks * ctx->g.bs > 0x7fffffffull) return B200KV_EINVAL;
   DeviceGuard dg(ctx->cfg.device);
   std::lock_guard<std::mutex> lk(ctx->mu);
+  std::vector<uint64_t> bases;
+  const int rc = plane_bases(ctx->g, k_ptrs, v_ptrs, &bases);
+  if (rc) return rc;
   if (peer_device != ctx->cfg.device) {
     int can = 0;
     CU_TRY(cudaDeviceCanAccessPeer(&can, ctx->cfg.device, peer_device));
@@ -1779,20 +1788,8 @@ extern "C" int b200kv_import_peer_ptrs(b200kv_ctx* ctx, int32_t peer_id, int32_t
     }
     cudaGetLastError();
   }
-  const uint32_t ppl = ctx->g.planes_per_layer;
-  std::vector<uint64_t> bases(ctx->g.planes);
-  for (uint32_t l = 0; l < ctx->g.L; ++l) {
-    for (uint32_t kv = 0; kv < ppl; ++kv) {
-      bases[ppl * l + kv] = reinterpret_cast<uint64_t>(kv ? v_ptrs[l] : k_ptrs[l]);
-      if (!bases[ppl * l + kv] || bases[ppl * l + kv] % 16) return B200KV_EINVAL;
-    }
-  }
-  std::vector<uint64_t> idx_bases;   // an engine with indexer planes takes the peer's in v_ptrs
-  for (uint32_t l = 0; ctx->g.indexed && l < ctx->g.L; ++l) {
-    idx_bases.push_back(reinterpret_cast<uint64_t>(v_ptrs[l]));
-    if (!idx_bases.back() || idx_bases.back() % 16) return B200KV_EINVAL;
-  }
-  return install_peer(ctx, peer_id, peer_device, bases, peer_block_stride_bytes, peer_n_blocks, {}, idx_bases);
+  std::vector<void*> none;   // raw pointers: no mappings to close
+  return install_peer(ctx, peer_id, peer_device, bases, peer_block_stride_bytes, peer_n_blocks, &none);
 }
 
 extern "C" int b200kv_peer_pull_async(b200kv_ctx* ctx, int32_t peer_id, const int64_t* src_slots,

@@ -48,7 +48,7 @@
 namespace b200kv {
 
 struct PagedSide {
-  const uint64_t* bases;  // device array [2*L]: K plane of layer l at [2l], V plane at [2l+1]; MLA: [L] latent planes
+  const uint64_t* bases;  // device array: K plane of layer l at [2l], V at [2l+1]; MLA: latent (or indexer) at [l]
   uint64_t block_stride;  // bytes between consecutive blocks of one plane
   uint32_t block_tokens;
   uint32_t token_bytes;   // H*D*elem (NHD: one token's heads are contiguous)
