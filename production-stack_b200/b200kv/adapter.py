@@ -204,8 +204,10 @@ class SchedulerState:
 
     def __init__(self, lookup, block_size: int, chunk: int, discard_partial_chunks: bool,
                  save_decode_cache: bool = False, kv_role: str = "kv_both", async_load: bool = False,
-                 priority_limit: int | None = None):
+                 priority_limit: int | None = None, draft_layers: int = 0):
         self.lookup = lookup
+        # attention layers of a speculative-decoding drafter in the stored chunks (num_new_matched_tokens)
+        self.draft_layers = draft_layers
         # requests whose priority value exceeds the limit are served from the cache but not saved
         # (adapter :1163, :1332-1337: `request_priority > config.priority_limit`)
         self.priority_limit = priority_limit
@@ -248,10 +250,26 @@ class SchedulerState:
         self.num_hit_tokens += hit
         self.num_requested_tokens += len(prompt_token_ids)
         need = hit - num_computed_tokens
-        if hit == num_tokens and not self.async_load:
+        if self.draft_layers:
+            hit = self._draft_hit(hit)
+            # A drafter's KV at position i comes from the target's hidden state at i and token i+1.  At hit-1 the
+            # stored draft KV used the storing request's token hit, which no chunk key covers: report one token
+            # less, still load all `hit`, and vLLM recomputes position hit-1 in the target and the drafter.  This
+            # also recomputes the last token of a full-prompt hit, so nothing else is subtracted (async included).
+            need = hit - num_computed_tokens - 1
+        elif hit == num_tokens and not self.async_load:
             need -= 1  # full-prompt hit: vLLM must still compute the last token
         self.load_specs[req_id] = LoadSpec(num_computed_tokens, hit, False)
         return max(need, 0)
+
+    def _draft_hit(self, hit: int) -> int:
+        """The tokens to load when the one before the last is reported as the hit.  A detached load gets blocks for
+        the reported tokens only, so the last loaded position, hit-1, must share a block with position hit-2.  A
+        whole-chunk hit does (C % bs == 0); one that ends in a partial chunk with hit ≡ 1 (mod bs) does not, and
+        is trimmed to its whole chunks."""
+        while self.async_load and hit > 0 and (hit - 1) % self.block_size == 0:
+            hit = (hit - 1) // self.chunk * self.chunk
+        return hit
 
     # update_state_after_alloc (adapter :1231-1293)
     def after_alloc(self, request, num_external_tokens: int, block_ids=None):

@@ -78,7 +78,9 @@ def geometry_from_vllm(vllm_config, cfg: B200KVConfig, n_blocks: int = 1) -> KVG
     named by "float16" / "bfloat16"; every other cache dtype (fp8*, ...) keeps bf16, which only RAW reads.
     An MLA model with DeepSeek Sparse Attention (DeepSeek-V3.2: index_topk in the HF config, vLLM's test) also
     has an indexer key cache per layer, which the geometry's indexer planes describe.  With the fp8_ds_mla cache a
-    latent token is already a 656-byte FP8 record, so the chunk stores it RAW, also when FP8 is asked for."""
+    latent token is already a 656-byte FP8 record, so the chunk stores it RAW, also when FP8 is asked for.
+    With speculative decoding by a drafter that owns attention layers (draft_layers_of), those layers follow the
+    target's: n_layers counts both."""
     mc, pc, cc = vllm_config.model_config, vllm_config.parallel_config, vllm_config.cache_config
     dt = str(cc.cache_dtype)
     dtype = _lib.DTYPE_BF16
@@ -99,7 +101,9 @@ def geometry_from_vllm(vllm_config, cfg: B200KVConfig, n_blocks: int = 1) -> KVG
             _log_once("b200kv: the fp8_ds_mla cache already holds FP8 latent records: chunks are stored RAW")
     hf = getattr(mc, "hf_text_config", None) or getattr(mc, "hf_config", None)
     sparse = mla and hasattr(hf, "index_topk")   # vLLM's own test for a V3.2 model (deepseek_v2.py, is_v32)
-    return KVGeometry(n_layers=mc.get_num_layers(pc), n_kv_heads=1 if mla else mc.get_num_kv_heads(pc),
+    draft = draft_layers_of(vllm_config)
+    return KVGeometry(n_layers=mc.get_num_layers(pc) + draft, draft_layers=draft,
+                      n_kv_heads=1 if mla else mc.get_num_kv_heads(pc),
                       head_dim=head_dim, n_blocks=n_blocks, block_tokens=cc.block_size,
                       chunk_tokens=cfg.chunk_size, elem_bytes=elem, block_stride_bytes=0, fmt=fmt,
                       layout=_lib.LAYOUT_MLA if mla else _lib.LAYOUT_NHD, dtype=dtype,
@@ -111,10 +115,63 @@ MLA_FP8_DS_BYTES = 656   # one token of vLLM's fp8_ds_mla latent cache (uint8): 
 _LOGGED: set[str] = set()
 
 
+def draft_layers_of(vllm_config) -> int:
+    """Attention layers a speculative-decoding drafter adds to the target's KV-cache group.  vLLM puts them there
+    (validate_same_kv_cache_group, v1/spec_decode/llm_base_proposer.py) and names them from num_hidden_layers
+    upwards (DeepSeekMultiTokenPredictor.mtp_start_layer_idx; start_layer_id in llama_eagle.py / llama_eagle3.py).
+    MTP ("mtp" and the per-model aliases vLLM folds into it): the model's num_nextn_predict_layers / n_predict.
+    EAGLE and EAGLE-3: the draft model's layer count.  Every other method (ngram, suffix, ...) and no speculative
+    config: 0."""
+    sc = getattr(vllm_config, "speculative_config", None)
+    method = str(getattr(sc, "method", None) or "")
+    if sc is None or not (method == "mtp" or method.endswith("_mtp") or method in ("eagle", "eagle3")):
+        return 0
+    dmc = getattr(sc, "draft_model_config", None)
+    hf = getattr(dmc, "hf_config", None)
+    if method in ("eagle", "eagle3"):
+        n = getattr(hf, "num_hidden_layers", None)
+    else:
+        n = getattr(hf, "n_predict", None) or getattr(hf, "num_nextn_predict_layers", None)
+        if not n:
+            mc = vllm_config.model_config
+            thf = getattr(mc, "hf_text_config", None) or getattr(mc, "hf_config", None)
+            n = getattr(thf, "num_nextn_predict_layers", None)
+    if not n or int(n) < 0:
+        raise ValueError(f"speculative method {method!r}: cannot tell how many attention layers the drafter has")
+    if int(getattr(vllm_config.parallel_config, "pipeline_parallel_size", 1) or 1) > 1:
+        # only the last stage holds the drafter, so the stages' caches would differ in more than their layer range
+        raise ValueError(f"B200KVConnector does not support speculative decoding ({method!r}, {int(n)} draft "
+                         "layers) with pipeline parallelism")
+    return int(n)
+
+
 def _log_once(msg: str):
     if msg not in _LOGGED:
         _LOGGED.add(msg)
         logger.info(msg)
+
+
+def _layer_index_of(name: str) -> int:
+    """vLLM's layer index of a KV-cache layer name ("model.layers.61.self_attn.attn" -> 61)."""
+    from vllm.model_executor.models.utils import extract_layer_index
+    try:
+        return extract_layer_index(name)
+    except (AssertionError, ValueError) as e:
+        raise ValueError(f"KV cache {name}: no layer index in the name") from e
+
+
+def hook_waits(layer: int, n_target: int, n_layers: int, layers_per_group: int, wait_ahead: bool) -> list[int]:
+    """Layers whose load groups target layer `layer`'s wait_for_layer_load waits for (b200kv_wait_layer waits for
+    the group holding the layer): its own group where it starts; with wait_ahead the next target layer's group where
+    it starts; and in the last target layer's hook every group that starts at a draft layer.  A draft layer in the
+    last target layer's group is covered by that group's wait."""
+    G = layers_per_group
+    waits = [layer] if layer % G == 0 else []
+    if wait_ahead and (layer + 1) % G == 0 and layer + 1 < n_target:
+        waits.append(layer + 1)
+    if layer == n_target - 1:
+        waits += [l for l in range(n_target, n_layers) if l % G == 0]
+    return waits
 
 
 def owner_tag_of(instance_id: str) -> int:
@@ -184,6 +241,7 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
         self._engine: KVEngine | None = None
         self._worker: WorkerState | None = None
         self._wait_ahead, self._n_layers = False, 0   # layer-wise waits one layer ahead (register_kv_caches)
+        self._n_target = 0                            # layers before the draft layers (register_kv_caches)
         self._sched: SchedulerState | None = None
         self._controller = None
         self._engine_id = str(ktc.engine_id or "engine")
@@ -223,7 +281,7 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
 
             self._sched = SchedulerState(lookup, self._block_size, self._chunk, self._discard_partial,
                                          self.cfg.save_decode_cache, self.kv_role, async_load=self.cfg.async_load,
-                                         priority_limit=self.cfg.priority_limit)
+                                         priority_limit=self.cfg.priority_limit, draft_layers=geom.draft_layers)
             if self.kv_role != "kv_producer":     # the scheduler fetches every TP rank's chunks of a prompt
                 # (one seed for MLA: every rank loads the same latent chunks)
                 self._remote = self._make_remote(list(dict.fromkeys(self._key_seed(r) for r in range(self._world))))
@@ -265,24 +323,39 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
         """KVConnectorBase_V1.register_kv_caches (base.py:251) — adapter :786-795."""
         if not kv_caches:
             raise ValueError("no KV cache tensors to register")
+        # Layer order is the layer index, not the dict's order: the target's layers 0..L-1, then a drafter's
+        # L..L+D-1 (vLLM puts them in the same group).  A stable sort keeps DeepSeek-V3.2's indexer caches in the
+        # same order as the latent ones.
+        kv_caches = dict(sorted(kv_caches.items(), key=lambda kv: _layer_index_of(kv[0])))
         # DeepSeek-V3.2: the latent layers and the indexer caches of the same layers come in one group
         tensors, idx = split_indexer_caches(kv_caches)
         t0 = tensors[0]
         k, v, stride, nb, h, d, tile_layout = paged_layout_of(t0, self._block_size)
         geom0 = geometry_from_vllm(self._vllm_config, self.cfg)
+        # only the attention layers call wait_for_layer_load: the hook is keyed by the latent layers' names
+        lat_names = [n for n, t in kv_caches.items() if not any(t is x for x in idx)]
+        if geom0.draft_layers:
+            L, D = geom0.target_layers, geom0.draft_layers
+            drafts = [i for i in map(_layer_index_of, lat_names) if i >= L]
+            if drafts != list(range(L, L + D)):
+                raise ValueError(f"KV cache tensors do not match the model geometry: the speculative config implies "
+                                 f"{D} draft layer(s) with indices {L}..{L + D - 1} after the {L} target layers, the "
+                                 f"registered layers have {len(drafts)} at or above index {L}: {drafts}")
         geom = KVGeometry(n_layers=len(tensors), n_kv_heads=h, head_dim=d, n_blocks=nb,
                           block_tokens=self._block_size, chunk_tokens=self._chunk,
                           elem_bytes=t0.element_size(), block_stride_bytes=stride, fmt=geom0.fmt,
                           layout=tile_layout, dtype=dtype_code(t0.dtype) or _lib.DTYPE_BF16,
                           idx_value_bytes=INDEXER_VALUE_BYTES if idx else 0,
                           idx_scale_bytes=INDEXER_SCALE_BYTES if idx else 0,
-                          idx_block_stride_bytes=idx[0].stride(0) if idx else 0)
+                          idx_block_stride_bytes=idx[0].stride(0) if idx else 0,
+                          draft_layers=geom0.draft_layers)
         if geom.indexed != geom0.indexed:
             raise ValueError("KV cache tensors " + ("include" if idx else "lack") + " indexer caches, which the "
                              "model config " + ("does not imply" if idx else "implies"))
         if geom.chunk_bytes != geom0.chunk_bytes:
             raise ValueError("KV cache tensors do not match the model geometry the pool was sized for "
-                             f"({geom.chunk_bytes} vs {geom0.chunk_bytes} bytes per chunk)")
+                             f"({geom.chunk_bytes} vs {geom0.chunk_bytes} bytes per chunk, {len(tensors)} vs "
+                             f"{geom0.n_layers} layers of which {geom0.draft_layers} draft layers)")
         if geom.dtype != geom0.dtype:   # the key seed is derived from the vLLM config's type
             raise ValueError(f"KV cache dtype {t0.dtype} differs from the one the vLLM config implies")
         rank = getattr(self._vllm_config.parallel_config, "rank", 0)
@@ -295,10 +368,8 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
                                 numa_policy=_lib.NUMA_INTERLEAVE if self.cfg.pool_name else _lib.NUMA_LOCAL)
         logger.info("b200kv pool pages: %s", self._engine.numa_placement())
         self._engine.register_kv_caches(kv_caches if idx else tensors)
-        # only the attention layers call wait_for_layer_load: the hook is keyed by the latent layers' names
-        lat_names = [n for n, t in kv_caches.items() if not any(t is x for x in idx)]
         self._layer_index = {name: i for i, name in enumerate(lat_names)}
-        self._n_layers = len(lat_names)
+        self._n_layers, self._n_target = len(lat_names), geom.target_layers
         # DeepSeek-V3.2 runs layer l's indexer, which reads the indexer keys of layer l, BEFORE layer l's attention
         # calls wait_for_layer_load; the indexer calls no connector hook.  Layer-wise loads then wait one layer
         # ahead: layer 0's group in start_load_kv, layer l+1's group in layer l's hook.
@@ -339,7 +410,8 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
                 self._chunk, owner_tag=owner_tag_of(self.cfg.instance_id) if self.cfg.pool_name else 0,
                 include_partial=not self._discard_partial, heartbeat_s=self.cfg.worker_heartbeat_s,
                 ip=self.cfg.advertise_ip)
-        logger.info("b200kv registered %d layers, %d blocks, stride %d", len(tensors), nb, stride)
+        logger.info("b200kv registered %d layers (%d draft), %d blocks, stride %d", len(tensors), geom.draft_layers,
+                    nb, stride)
 
     def _tp_rank(self) -> int:
         """This worker's tensor-parallel rank (every rank of an engine shares the engine id)."""
@@ -377,19 +449,19 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
         """Chunk-wise loads are ordered before the forward pass by a stream wait.  Layer-wise loads
         (B200KV_LAYERWISE=1; LMCache `use_layerwise`, adapter :907-929): the compute stream waits
         here, once per layer group, while later groups are still crossing PCIe.  With indexer caches (DeepSeek-V3.2)
-        the wait runs one layer ahead: the next layer's indexer reads its keys before that layer's hook runs."""
+        the wait runs one layer ahead: the next layer's indexer reads its keys before that layer's hook runs.
+        A speculative-decoding drafter runs right after the last target layer, on the same stream, and its own hooks
+        may not run (CUDA-graph replay): the last target layer's hook also waits for every group holding a draft
+        layer, both planes of each included, and a draft layer's hook does nothing."""
         w = self._worker
         if w is None or not w.layer_loads:
             return
         idx = self._layer_index.get(layer_name)
-        if idx is None:
+        if idx is None or idx >= self._n_target:
             return
         self._layer_hooks_seen += 1
-        G = self.cfg.layer_group
-        if idx % G == 0:
-            w.wait_layer(idx, torch.cuda.current_stream())
-        if self._wait_ahead and (idx + 1) % G == 0 and idx + 1 < self._n_layers:
-            w.wait_layer(idx + 1, torch.cuda.current_stream())
+        for l in hook_waits(idx, self._n_target, self._n_layers, self.cfg.layer_group, self._wait_ahead):
+            w.wait_layer(l, torch.cuda.current_stream())
 
     def save_kv_layer(self, layer_name: str, kv_layer: torch.Tensor, attn_metadata, **kwargs: Any) -> None:
         return  # whole-request store in wait_for_save: CUDA-graph replay skips per-layer hooks (base.py:591-611)

@@ -89,6 +89,18 @@ class KVGeometry:
     idx_value_bytes: int = 0
     idx_scale_bytes: int = 0
     idx_block_stride_bytes: int = 0
+    # speculative decoding (MTP, EAGLE, EAGLE-3): how many of the n_layers are the drafter's, which vLLM puts in the
+    # target's KV-cache group.  They are layers n_layers - draft_layers .. n_layers - 1, with the target's geometry.
+    draft_layers: int = 0
+
+    def __post_init__(self):
+        if not 0 <= self.draft_layers < max(self.n_layers, 1):
+            raise ValueError(f"{self.draft_layers} draft layers in a geometry of {self.n_layers} layers")
+
+    @property
+    def target_layers(self) -> int:
+        """Layers of the target model: the engine's layers before the draft layers."""
+        return self.n_layers - self.draft_layers
 
     @property
     def fp16(self) -> bool:
@@ -142,7 +154,9 @@ class KVGeometry:
         the same on every tensor-parallel rank, so its namespace keeps only the pipeline stage
         (rank // world_size) of the rank: one stored copy serves every rank of the stage.  An fp16 cache
         appends "|fp16", so its chunks (RAW included) never alias a bf16 replica's; bf16 seeds are unchanged.  A
-        geometry with indexer planes appends "|idx<bytes per token>" (V3.2: "|idx132"); others are unchanged."""
+        geometry with indexer planes appends "|idx<bytes per token>" (V3.2: "|idx132"); others are unchanged.
+        Draft layers count in n_layers, so a speculative-decoding replica's chunks, which carry the drafter's planes,
+        have a namespace of their own; a geometry without draft layers keeps its seed."""
         if self.mla:
             rank //= max(world_size, 1)
         tag = f"{model}|{world_size}|{rank}|{self.n_layers}|{self.n_kv_heads}|{self.head_dim}|" \

@@ -83,13 +83,18 @@ def _indexer_of(geom) -> int:
     return int(getattr(geom, "idx_token_bytes", 0))
 
 
+def _draft_of(geom) -> int:
+    """Draft layers among a geometry's layers (KVGeometry.draft_layers; 0 for a geometry without the field)."""
+    return int(getattr(geom, "draft_layers", 0))
+
+
 def publish_ipc(engine_id: str, engine, device: int, rank: int = 0, tp_size: int = 1) -> str:
     g = engine.geom
     doc = {"engine_id": engine_id, "device": device, "pid": os.getpid(), "rank": rank, "tp_size": tp_size,
            "n_blocks": g.n_blocks,
            "block_stride": g.stride, "n_layers": g.n_layers, "n_kv_heads": g.n_kv_heads, "head_dim": g.head_dim,
            "block_tokens": g.block_tokens, "elem_bytes": g.elem_bytes, "layout": g.layout, "dtype": _dtype_of(g),
-           "indexer": _indexer_of(g),
+           "indexer": _indexer_of(g), "draft_layers": _draft_of(g),
            "descs": base64.b64encode(engine.export_ipc()).decode()}
     path = ipc_path(engine_id, rank)
     tmp = path + f".{os.getpid()}.tmp"
@@ -140,7 +145,14 @@ class PeerResolver:
         g = self.engine.geom
         doc.setdefault("dtype", DTYPE_BF16)   # documents published before the field are bf16 caches
         doc.setdefault("indexer", 0)          # ... and caches without indexer planes
-        for k, mine in (("n_layers", g.n_layers), ("n_kv_heads", g.n_kv_heads), ("head_dim", g.head_dim),
+        doc.setdefault("draft_layers", 0)     # ... and replicas without a speculative-decoding drafter
+        if (doc["n_layers"], doc["draft_layers"]) != (g.n_layers, _draft_of(g)):
+            # a drafter's layers follow the target's in the cache: the pages of a replica with one are not those of
+            # a replica without one (or with another drafter)
+            raise ValueError(f"peer {remote_engine_id}: n_layers={doc['n_layers']} with {doc['draft_layers']} draft "
+                             f"layer(s) differs from local {g.n_layers} with {_draft_of(g)}: replicas pair only "
+                             "with the same speculative-decoding drafter, or both without one")
+        for k, mine in (("n_kv_heads", g.n_kv_heads), ("head_dim", g.head_dim),
                         ("block_tokens", g.block_tokens), ("elem_bytes", g.elem_bytes), ("layout", g.layout),
                         ("dtype", _dtype_of(g)), ("indexer", _indexer_of(g))):
             if doc[k] != mine:
