@@ -210,6 +210,14 @@ int b200kv_pool_get_stats(b200kv_pool* pool, b200kv_pool_stats* out);
  * b200kv_pool_check verifies those structures against the slot array (0, or -EIO).          */
 int b200kv_pool_check(b200kv_pool* pool);
 int b200kv_pool_clear(b200kv_pool* pool); /* KVConnectorBase_V1.reset_cache               */
+/* Index rebuild (the disk tier's index after a restart): entry i puts keys[i] READY into slot slots[i], with its
+ * token count, format tag and owner, appended to the LRU tail in the order given (oldest first).  An entry whose
+ * slot is out of range or not free, whose key is already present, or whose n_tokens <= 0 is skipped.  Returns the
+ * number of entries placed (>= 0) or a negative error.                                      */
+int b200kv_pool_place(b200kv_pool* pool, const uint32_t* slots, const uint64_t* keys, const int32_t* n_tokens,
+                      const uint32_t* fmts, const uint32_t* owners, int32_t n);
+/* Remove one READY chunk (a reader found it corrupt).  -EBUSY while it is pinned, -ENOENT if absent. */
+int b200kv_pool_drop(b200kv_pool* pool, uint64_t key);
 
 /* ======================================================================================= */
 /* engine group (CUDA, sm_90a)                                                              */
@@ -437,6 +445,52 @@ int b200kv_remote_put(b200kv_remote* r, b200kv_pool* local, uint64_t key, uint32
 int b200kv_remote_get(b200kv_remote* r, b200kv_pool* local, uint64_t key, uint32_t owner);
 int b200kv_remote_stats(b200kv_remote* r, b200kv_pool_stats* out);
 int b200kv_remote_traffic(b200kv_remote* r, uint64_t* bytes_up, uint64_t* bytes_down);
+
+/* ======================================================================================= */
+/* disk group (CPU only): the local-disk tier                                               */
+/* ======================================================================================= */
+/* LMCACHE_LOCAL_DISK / LMCACHE_MAX_LOCAL_DISK_SIZE (helm/templates/deployment-vllm-multi.yaml:334-337): chunks
+ * below the pinned pool, on local NVMe.  One preallocated file per (directory, chunk size),
+ * <dir>/b200kv-disk-<chunk_bytes hex>.slots: a 4 KiB file header, then slots of a 4 KiB slot header (magic,
+ * version, key, format tag, token count, owner, payload length, XXH64 of the payload, write time, the file's
+ * UUID, XXH64 of the header) followed by the chunk rounded up to 4 KiB.  The index is a b200kv_pool in shm,
+ * named after the file, with pool slot i <-> file slot i; every process that opens the file shares it, and one
+ * that is new or describes another incarnation of the file is rebuilt from the slot headers.  O_DIRECT I/O
+ * (buffered with POSIX_FADV_DONTNEED where the filesystem refuses it).  A `b200kv_disk` may be used from several
+ * threads at once.                                                                          */
+typedef struct b200kv_disk b200kv_disk;
+typedef struct b200kv_disk_stats {
+  uint64_t n_slots, n_used;    /* disk slots, slots in use (shared by every opener)                    */
+  uint64_t slot_bytes;         /* bytes of one disk slot: 4 KiB header + chunk rounded up to 4 KiB     */
+  uint64_t n_put, n_get;       /* chunks written / read back into a pool by this handle               */
+  uint64_t n_get_miss;         /* gets of a key the index does not hold                               */
+  uint64_t n_corrupt;          /* slots rejected by a header or payload check (never loaded)          */
+  uint64_t n_evicted, n_dropped; /* index: LRU evictions; puts refused because every slot was pinned */
+  uint64_t bytes_written, bytes_read;
+  uint64_t hash_ns, copy_ns, io_ns; /* time in XXH64, in bounce-buffer copies, in pread/pwrite         */
+  uint64_t n_restored;         /* chunks the index rebuild at open found in the file                  */
+  int32_t direct_io;           /* 1: O_DIRECT, 0: buffered                                            */
+  int32_t last_errno;          /* errno of the most recent failed read or write                       */
+} b200kv_disk_stats;
+
+/* Opens (creating and preallocating it if needed) the file for chunks of chunk_bytes in the existing directory
+ * `dir`, sized to floor((disk_bytes - 4 KiB) / slot_bytes) slots; an existing file keeps its size.  -ENOENT /
+ * -ENOTDIR: no such directory; -EACCES / -EROFS: not writable; -ENOSPC: the preallocation does not fit.      */
+int b200kv_disk_open(const char* dir, uint64_t disk_bytes, uint64_t chunk_bytes, b200kv_disk** out);
+int b200kv_disk_close(b200kv_disk* disk);
+/* Local pool -> disk.  -ENOENT: not READY locally; -EEXIST: on disk already; -ENOSPC: every disk slot is
+ * pinned or being written; -EIO: the write failed (stats.last_errno says why).              */
+int b200kv_disk_put(b200kv_disk* disk, b200kv_pool* local, uint64_t key, uint32_t owner);
+/* Disk -> local pool: pin the disk slot, reserve a pool slot, read, verify, commit.  OK also when the chunk is
+ * already local.  -ENOENT: not on disk, or it failed its check (then it is dropped from the index);
+ * -ENOSPC: no local slot could be freed; -EIO: the read failed.                              */
+int b200kv_disk_get(b200kv_disk* disk, b200kv_pool* local, uint64_t key);
+/* *n_prefix = how many leading keys the disk holds.                                          */
+int b200kv_disk_lookup(b200kv_disk* disk, const uint64_t* keys, int32_t n_keys, int32_t* n_prefix);
+int b200kv_disk_get_stats(b200kv_disk* disk, b200kv_disk_stats* out);
+/* Empties the index and retires every slot header on disk (KVConnectorBase_V1.reset_cache); -EBUSY if a chunk
+ * was pinned or being written and stayed.                                                     */
+int b200kv_disk_clear(b200kv_disk* disk);
 
 #ifdef __cplusplus
 }

@@ -21,6 +21,7 @@ POOL_CREATE, POOL_ATTACH, POOL_CREATE_OR_ATTACH = 1, 2, 3
 NUMA_LOCAL, NUMA_INTERLEAVE, NUMA_OFF = 0, 1, 2
 
 OK, EINVAL, ENOMEM, ENODEV, ENOENT, EEXIST, ENOSPC, ENOTSUP, EBUSY = 0, -22, -12, -19, -2, -17, -28, -95, -16
+EIO = -5
 
 
 class PoolConfig(C.Structure):
@@ -33,6 +34,16 @@ class PoolStats(C.Structure):
         "n_slots", "n_used", "slot_bytes", "n_lookups", "n_lookup_chunks", "n_hit_chunks",
         "n_hit_tokens", "n_requested_tokens", "n_stored_chunks", "n_evicted_chunks",
         "n_dropped_chunks", "n_reclaimed_chunks", "n_recoveries")]
+
+    def as_dict(self):
+        return {n: int(getattr(self, n)) for n, _ in self._fields_}
+
+
+class DiskStats(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in (
+        "n_slots", "n_used", "slot_bytes", "n_put", "n_get", "n_get_miss", "n_corrupt", "n_evicted", "n_dropped",
+        "bytes_written", "bytes_read", "hash_ns", "copy_ns", "io_ns", "n_restored")] + [
+        ("direct_io", C.c_int32), ("last_errno", C.c_int32)]
 
     def as_dict(self):
         return {n: int(getattr(self, n)) for n, _ in self._fields_}
@@ -91,6 +102,8 @@ SIGNATURES = {
     "b200kv_pool_get_stats": (C.c_int, [_P, C.POINTER(PoolStats)]),
     "b200kv_pool_clear": (C.c_int, [_P]),
     "b200kv_pool_check": (C.c_int, [_P]),
+    "b200kv_pool_place": (C.c_int, [_P, _U32P, _U64P, _I32P, _U32P, _U32P, C.c_int32]),
+    "b200kv_pool_drop": (C.c_int, [_P, C.c_uint64]),
     "b200kv_engine_create": (C.c_int, [C.POINTER(EngineConfig), _P, C.POINTER(_P)]),
     "b200kv_engine_destroy": (C.c_int, [_P]),
     "b200kv_set_cache_dtype": (C.c_int, [_P, C.c_int32]),
@@ -133,6 +146,13 @@ SIGNATURES = {
     "b200kv_remote_get": (C.c_int, [_P, _P, C.c_uint64, C.c_uint32]),
     "b200kv_remote_stats": (C.c_int, [_P, C.POINTER(PoolStats)]),
     "b200kv_remote_traffic": (C.c_int, [_P, _U64P, _U64P]),
+    "b200kv_disk_open": (C.c_int, [C.c_char_p, C.c_uint64, C.c_uint64, C.POINTER(_P)]),
+    "b200kv_disk_close": (C.c_int, [_P]),
+    "b200kv_disk_put": (C.c_int, [_P, _P, C.c_uint64, C.c_uint32]),
+    "b200kv_disk_get": (C.c_int, [_P, _P, C.c_uint64]),
+    "b200kv_disk_lookup": (C.c_int, [_P, _U64P, C.c_int32, _I32P]),
+    "b200kv_disk_get_stats": (C.c_int, [_P, C.POINTER(DiskStats)]),
+    "b200kv_disk_clear": (C.c_int, [_P]),
 }
 
 _lib = None

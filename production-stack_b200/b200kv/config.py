@@ -7,6 +7,7 @@ from __future__ import annotations
 
 import logging
 import os
+import tempfile
 from dataclasses import dataclass, field
 
 from ._lib import FMT_FP8, FMT_Q4, FMT_RAW
@@ -16,8 +17,7 @@ logger = logging.getLogger("b200kv")
 _TRUE = {"1", "true", "yes", "on"}
 
 # accepted for compatibility but without effect here (out of scope rows of SURVEY.md Appendix A)
-_IGNORED = ("LMCACHE_MAX_LOCAL_DISK_SIZE", "LMCACHE_LOCAL_DISK",
-            "LMCACHE_ENABLE_NIXL", "LMCACHE_NIXL_ROLE", "LMCACHE_USE_EXPERIMENTAL")
+_IGNORED = ("LMCACHE_ENABLE_NIXL", "LMCACHE_NIXL_ROLE", "LMCACHE_USE_EXPERIMENTAL")
 
 
 def _b(v: str | None, default: bool) -> bool:
@@ -53,6 +53,9 @@ class B200KVConfig:
     device_tier_gb: float = 0.0           # B200KV_DEVICE_TIER_GB: HBM kept as a chunk cache peers can pull from (0 = off)
     remote_url: str | None = None         # LMCACHE_REMOTE_URL=lm://host:port: cache-server tier (b200kv/remote.py)
     remote_wait_ms: int = 2000            # B200KV_REMOTE_WAIT_MS: longest a request waits for its remote prefetch
+    local_disk: str | None = None         # LMCACHE_LOCAL_DISK: file:///dir/, /dir, or True (a directory under $TMPDIR)
+    max_local_disk_size: float = 0.0      # LMCACHE_MAX_LOCAL_DISK_SIZE (GB); the disk tier needs both (b200kv/disk.py)
+    disk_wait_ms: int = 2000              # B200KV_DISK_WAIT_MS: longest a request waits for its disk prefetch
     extra: dict = field(default_factory=dict)
 
     @staticmethod
@@ -98,6 +101,14 @@ class B200KVConfig:
         c.device_tier_gb = float(e.get("B200KV_DEVICE_TIER_GB", c.device_tier_gb))
         c.remote_url = e.get("LMCACHE_REMOTE_URL") or None
         c.remote_wait_ms = int(e.get("B200KV_REMOTE_WAIT_MS", c.remote_wait_ms))
+        c.local_disk = e.get("LMCACHE_LOCAL_DISK") or None
+        c.max_local_disk_size = float(e.get("LMCACHE_MAX_LOCAL_DISK_SIZE") or 0)
+        c.disk_wait_ms = int(e.get("B200KV_DISK_WAIT_MS", c.disk_wait_ms))
+        if c.max_local_disk_size > 0 and not _disk_path_given(c.local_disk):
+            logger.warning("%s=%s is accepted for chart compatibility but has no effect in b200kv",
+                           "LMCACHE_MAX_LOCAL_DISK_SIZE", e.get("LMCACHE_MAX_LOCAL_DISK_SIZE"))
+        elif _disk_path_given(c.local_disk) and c.max_local_disk_size <= 0:
+            logger.warning("LMCACHE_LOCAL_DISK=%s has no effect without LMCACHE_MAX_LOCAL_DISK_SIZE > 0", c.local_disk)
         for k in _IGNORED:
             if e.get(k) not in (None, "", "0", "False", "false"):
                 logger.warning("%s=%s is accepted for chart compatibility but has no effect in b200kv", k, e.get(k))
@@ -126,3 +137,31 @@ class B200KVConfig:
     @property
     def pool_bytes(self) -> int:
         return int(self.max_local_cpu_size_gb * (1 << 30))
+
+    @property
+    def disk_bytes(self) -> int:
+        """LMCACHE_MAX_LOCAL_DISK_SIZE in bytes, GB read as GiB like LMCACHE_MAX_LOCAL_CPU_SIZE (pool_bytes)."""
+        return int(self.max_local_disk_size * (1 << 30))
+
+    def disk_dir(self) -> str | None:
+        """The disk tier's directory, or None when the tier is off (it needs LMCACHE_LOCAL_DISK and a size > 0).
+        `file:///dir/` and `/dir` name it; True / 1 (what the operator emits) means default_disk_dir()."""
+        if self.max_local_disk_size <= 0 or not _disk_path_given(self.local_disk):
+            return None
+        v = str(self.local_disk).strip()
+        if v.lower() in _TRUE:
+            return default_disk_dir()
+        if v.startswith("file://"):
+            v = v[len("file://"):]
+        if "://" in v or not v.startswith("/"):
+            raise ValueError(f"LMCACHE_LOCAL_DISK={self.local_disk!r}: expected file:///dir/, /dir or True")
+        return v
+
+
+def default_disk_dir() -> str:
+    """Where LMCACHE_LOCAL_DISK=True puts the disk tier: b200kv-disk under $TMPDIR (/tmp by default)."""
+    return os.path.join(tempfile.gettempdir(), "b200kv-disk")
+
+
+def _disk_path_given(v) -> bool:
+    return v is not None and str(v).strip().lower() not in ("", "0", "false", "no", "off", "none")

@@ -68,6 +68,8 @@ class B200KVConnectorMetadata(KVConnectorMetadata):
     # this engine's cumulative (lookups, hit tokens, requested tokens): the worker reports them as the
     # lmcache:* series, so replicas sharing one pool each report their own traffic, not the box's
     sched_counters: tuple = (0, 0, 0)
+    # this engine's scheduler's cumulative disk-tier (fetched, corrupt) chunks: the scheduler reads the disk
+    disk_counters: tuple = (0, 0)
 
 
 def geometry_from_vllm(vllm_config, cfg: B200KVConfig, n_blocks: int = 1) -> KVGeometry:
@@ -249,6 +251,10 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
         self._pdw: PDWorker | None = None
         self._remote_computed: dict[str, int] = {}
         self._remote = None     # cache-server tier (LMCACHE_REMOTE_URL), b200kv/remote.py
+        self._disk = None       # local-disk tier (LMCACHE_LOCAL_DISK), b200kv/disk.py
+        self._disk_dir = self.cfg.disk_dir()       # None: no disk tier (a malformed value raises here)
+        self._disk_prefetch = False                # scheduler: prefetch from the disk tier (not on a kv_producer)
+        self._disk_counters: tuple = (0, 0)        # worker: last disk counters received from this engine's scheduler
         self._sched_counters: tuple = (0, 0, 0)   # worker: last counters received from this engine's scheduler
         if role == KVConnectorRole.SCHEDULER:
             self._pd = PDScheduler(self._engine_id, self._block_size,
@@ -282,9 +288,13 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
             self._sched = SchedulerState(lookup, self._block_size, self._chunk, self._discard_partial,
                                          self.cfg.save_decode_cache, self.kv_role, async_load=self.cfg.async_load,
                                          priority_limit=self.cfg.priority_limit, draft_layers=geom.draft_layers)
-            if self.kv_role != "kv_producer":     # the scheduler fetches every TP rank's chunks of a prompt
-                # (one seed for MLA: every rank loads the same latent chunks)
-                self._remote = self._make_remote(list(dict.fromkeys(self._key_seed(r) for r in range(self._world))))
+            # the scheduler fetches every TP rank's chunks of a prompt (one seed for MLA: every rank loads the same
+            # latent chunks); a kv_producer's scheduler keeps its disk tier for reset_cache only
+            seeds = list(dict.fromkeys(self._key_seed(r) for r in range(self._world)))
+            self._disk = self._make_disk(seeds)
+            self._disk_prefetch = self._disk is not None and self.kv_role != "kv_producer"
+            if self.kv_role != "kv_producer":
+                self._remote = self._make_remote(seeds)
             if not self.cfg.pool_name:
                 # a per-engine segment dies with its engine (vLLM's engine ids are random: nobody would
                 # ever attach to it again); a named, shared one stays for the other replicas of the box
@@ -304,6 +314,30 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
         logger.info("b200kv remote tier: %s:%d", *hp)
         return RemoteTier(self._pool, hp[0], hp[1], self._chunk, key_seeds, owner=owner_tag_of(self.cfg.instance_id),
                           include_partial=not self._discard_partial, wait_s=self.cfg.remote_wait_ms / 1e3)
+
+    def _make_disk(self, key_seeds):
+        """LMCACHE_LOCAL_DISK + LMCACHE_MAX_LOCAL_DISK_SIZE (deployment-vllm-multi.yaml:334-337): the local-disk
+        tier behind the pinned pool.  A malformed value is a fatal misconfiguration; a directory that cannot hold
+        the tier is a warning, and the engine runs without it."""
+        d = self._disk_dir
+        if d is None:
+            return None
+        from .config import default_disk_dir
+        from .disk import DiskTier
+        try:
+            if d == default_disk_dir():
+                os.makedirs(d, exist_ok=True)
+                logger.info("b200kv disk tier: LMCACHE_LOCAL_DISK=%s, using %s", self.cfg.local_disk, d)
+            tier = DiskTier(self._pool, d, self.cfg.disk_bytes, self._chunk, key_seeds,
+                            owner=owner_tag_of(self.cfg.instance_id), include_partial=not self._discard_partial,
+                            wait_s=self.cfg.disk_wait_ms / 1e3, prefix_lease_ms=self.cfg.lookup_lease_ms)
+        except Exception as e:
+            logger.warning("b200kv disk tier in %s unavailable (%s); running without it", d, e)
+            return None
+        st = tier.file.stats()
+        logger.info("b200kv disk tier: %s, %d chunk slots (%.1f GB), %d chunks restored, %s I/O", d, st["n_slots"],
+                    st["n_slots"] * st["slot_bytes"] / 1e9, st["n_restored"], "direct" if st["direct_io"] else "buffered")
+        return tier
 
     def _key_seed(self, rank: int) -> int:
         """Same namespace in both roles: derived from the vLLM config only (the tile layout is a
@@ -395,8 +429,12 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
                 self._worker.tiers = self._worker.local_tier = None
         if self.kv_role != "kv_consumer":
             self._remote = self._make_remote(self._engine.key_seed)
-            if self._remote is not None:
-                self._worker.on_stored = self._remote.push     # upload what this worker stores
+            self._disk = self._make_disk(self._engine.key_seed)
+            hooks = [t.push for t in (self._disk, self._remote) if t is not None]   # write through / upload
+            if len(hooks) == 1:
+                self._worker.on_stored = hooks[0]
+            elif hooks:
+                self._worker.on_stored = lambda keys: [h(keys) for h in hooks]
         try:
             tp_rank = self._tp_rank()
             publish_ipc(self._engine_id, self._engine, t0.device.index or 0, tp_rank, self._world)   # peers may pull from us
@@ -434,6 +472,7 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
         md = self._get_connector_metadata()
         if isinstance(md, B200KVConnectorMetadata) and md.sched_counters[0] >= self._sched_counters[0]:
             self._sched_counters = tuple(md.sched_counters)
+            self._disk_counters = tuple(md.disk_counters)
         if self._pdw is not None and isinstance(md, B200KVConnectorMetadata) and (md.pd.pulls or md.pd.held):
             self._pdw.start_pulls(md.pd, stream=stream)
         self._layer_hooks_seen = 0
@@ -516,6 +555,13 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
                "num_requested_tokens": self._sched_counters[2] if getattr(self, "_rank", 0) == 0 else 0,
                "retrieve_bytes": ws.num_loaded_tokens * self._engine.geom.payload_bytes_per_token,
                "store_bytes": ws.num_stored_tokens * self._engine.geom.payload_bytes_per_token}
+        if self._disk_dir is not None:
+            ds = self._disk.stats() if self._disk is not None else {}
+            rank0 = getattr(self, "_rank", 0) == 0     # the scheduler's counters are per engine
+            cur.update({"disk_written_chunks": ds.get("written_chunks", 0),
+                        "disk_skipped_chunks": ds.get("skipped_chunks", 0),
+                        "disk_fetched_chunks": self._disk_counters[0] if rank0 else 0,
+                        "disk_corrupt_chunks": self._disk_counters[1] if rank0 else 0})
         prev = getattr(self, "_stats_prev", {})
         delta = {k: v - prev.get(k, 0) for k, v in cur.items()}
         self._stats_prev = cur
@@ -523,6 +569,8 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
             return None
         delta["local_cache_usage_bytes"] = ps["n_used"] * ps["slot_bytes"]
         delta["local_cache_capacity_bytes"] = ps["n_slots"] * ps["slot_bytes"]
+        if self._disk is not None:
+            delta["disk_usage_bytes"] = self._disk.stats()["usage_bytes"]
         return B200KVStats(delta)
 
     @classmethod
@@ -539,6 +587,9 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
         if self._remote is not None:
             self._remote.close()
             self._remote = None
+        if self._disk is not None:
+            self._disk.close()
+            self._disk = None
         if self._controller is not None:
             self._controller.close()
             self._controller = None
@@ -576,6 +627,11 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
         # multimodal items, cache_salt, LoRA adapter and lmcache.tag.* enter the chunk keys (adapter :1168-1172)
         ident = self._sched.identities.get(request.request_id) or request_identity(request)
         prompt = request.prompt_token_ids or []
+        # chunks on their way from the local disk, then from the cache server for what is still missing: ask again
+        # next step.  The disk's wait ends before the server's begins, so a request waits at most both budgets.
+        if self._disk_prefetch and self._disk.prefetch_state(
+                request.request_id, prompt if ident is None else ident.apply(prompt)) == self._disk.PENDING:
+            return None, False
         if self._remote is not None and self._remote.prefetch_state(
                 request.request_id, prompt if ident is None else ident.apply(prompt)) == self._remote.PENDING:
             return None, False   # chunks are on their way from the cache server: ask again next step
@@ -599,8 +655,12 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
     def build_connector_meta(self, scheduler_output: "SchedulerOutput") -> KVConnectorMetadata:
         assert self._sched is not None and self._pd is not None
         sc = self._sched
-        return B200KVConnectorMetadata(sc.build_meta(scheduler_output), self._pd.build_meta(),
-                                       (sc.num_lookups, sc.num_hit_tokens, sc.num_requested_tokens))
+        md = B200KVConnectorMetadata(sc.build_meta(scheduler_output), self._pd.build_meta(),
+                                     (sc.num_lookups, sc.num_hit_tokens, sc.num_requested_tokens))
+        if self._disk is not None:
+            ds = self._disk.stats()
+            md.disk_counters = (ds["fetched_chunks"], ds["corrupt_chunks"])
+        return md
 
     @_traced
     def request_finished(self, request: "Request", block_ids: list[int]) -> tuple[bool, dict[str, Any] | None]:
@@ -610,6 +670,8 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
         self._remote_computed.pop(request.request_id, None)   # looked up as a remote prefill but never allocated
         if self._remote is not None:
             self._remote.forget(request.request_id)
+        if self._disk is not None:
+            self._disk.forget(request.request_id)
         if self._pd is not None:
             ok = True
             st = getattr(request, "status", None)
@@ -628,4 +690,9 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
         return self.request_finished(request, block_ids[0] if block_ids else [])
 
     def reset_cache(self) -> bool | None:
-        return self._pool.clear() if self._pool is not None else None
+        if self._pool is None:
+            return None
+        ok = self._pool.clear()
+        if self._disk is not None:
+            ok = self._disk.clear() and ok
+        return ok

@@ -5,6 +5,9 @@ queries (helm/dashboards/lmcache-dashboard.json:204,295,389,453,517):
 
     lmcache:num_hit_tokens_total, lmcache:num_requested_tokens_total, lmcache:local_cache_usage,
     lmcache:retrieve_speed_{sum,count}   (+ store_speed, num_stored_tokens_total)
+
+With the local-disk tier on (LMCACHE_LOCAL_DISK), this build's own b200kv:disk_* series as well: disk_usage (bytes),
+disk_{fetched,written,skipped,corrupt}_chunks.
 """
 from __future__ import annotations
 
@@ -15,7 +18,9 @@ from vllm.distributed.kv_transfer.kv_connector.v1.metrics import KVConnectorProm
 
 _SUM_KEYS = ("num_hit_tokens", "num_requested_tokens", "num_stored_tokens", "num_loaded_tokens",
              "retrieve_seconds", "retrieve_calls", "retrieve_bytes", "store_bytes", "load_shortfalls",
-             "num_foreign_loaded_tokens", "num_tier_local_tokens", "num_tier_peer_tokens")
+             "num_foreign_loaded_tokens", "num_tier_local_tokens", "num_tier_peer_tokens",
+             "disk_fetched_chunks", "disk_written_chunks", "disk_skipped_chunks", "disk_corrupt_chunks")
+_DISK_COUNTERS = ("fetched", "written", "skipped", "corrupt")
 
 
 @dataclass
@@ -29,7 +34,7 @@ class B200KVStats(KVConnectorStats):
         for k in _SUM_KEYS:
             if k in other.data:
                 self.data[k] = self.data.get(k, 0) + other.data[k]
-        for k in ("local_cache_usage_bytes", "local_cache_capacity_bytes"):
+        for k in ("local_cache_usage_bytes", "local_cache_capacity_bytes", "disk_usage_bytes"):
             if k in other.data:
                 self.data[k] = other.data[k]  # gauges: last value wins
         return self
@@ -38,7 +43,8 @@ class B200KVStats(KVConnectorStats):
         d = self.data
         out: dict[str, int | float] = {k: d[k] for k in ("num_hit_tokens", "num_requested_tokens", "num_stored_tokens",
                                                           "num_loaded_tokens", "num_foreign_loaded_tokens", "num_tier_local_tokens",
-                                                          "num_tier_peer_tokens") if k in d}
+                                                          "num_tier_peer_tokens")
+                                        + tuple(f"disk_{c}_chunks" for c in _DISK_COUNTERS) if k in d}
         if d.get("retrieve_seconds"):
             out["retrieve_GBps"] = round(d.get("retrieve_bytes", 0) / d["retrieve_seconds"] / 1e9, 2)
         if "local_cache_usage_bytes" in d:
@@ -78,6 +84,16 @@ class B200KVPromMetrics(KVConnectorPromMetrics):
                                   labelnames=labelnames))
         self.r_cnt = per_engine(c(name="lmcache:retrieve_speed_count", documentation="number of retrieve calls",
                                   labelnames=labelnames))
+        self.disk = None
+        if _disk_enabled(vllm_config):
+            docs = {"fetched": "chunks read from the local disk tier into the pinned pool",
+                    "written": "chunks written through to the local disk tier",
+                    "skipped": "stored chunks not written to disk (queue full, no free disk slot, already evicted)",
+                    "corrupt": "disk chunks that failed their checksum (never loaded)"}
+            self.disk = {k: per_engine(c(name=f"b200kv:disk_{k}_chunks", documentation=docs[k], labelnames=labelnames))
+                         for k in _DISK_COUNTERS}
+            self.disk_usage = per_engine(g(name="b200kv:disk_usage", documentation="bytes of the local disk tier in use",
+                                           labelnames=labelnames, multiprocess_mode="mostrecent"))
 
     def observe(self, transfer_stats_data: dict[str, Any], engine_idx: int = 0):
         d = transfer_stats_data
@@ -89,6 +105,20 @@ class B200KVPromMetrics(KVConnectorPromMetrics):
         self.tier_peer[engine_idx].inc(d.get("num_tier_peer_tokens", 0))
         if "local_cache_usage_bytes" in d:
             self.usage[engine_idx].set(d["local_cache_usage_bytes"])
+        if self.disk is not None:
+            for k in _DISK_COUNTERS:
+                self.disk[k][engine_idx].inc(d.get(f"disk_{k}_chunks", 0))
+            if "disk_usage_bytes" in d:
+                self.disk_usage[engine_idx].set(d["disk_usage_bytes"])
         if d.get("retrieve_calls") and d.get("retrieve_seconds"):
             self.r_sum[engine_idx].inc(d.get("num_loaded_tokens", 0) / d["retrieve_seconds"] * d["retrieve_calls"])
             self.r_cnt[engine_idx].inc(d["retrieve_calls"])
+
+
+def _disk_enabled(vllm_config) -> bool:
+    from .config import B200KVConfig
+    try:
+        ktc = vllm_config.kv_transfer_config
+        return B200KVConfig.from_env().apply_extra(ktc.kv_connector_extra_config).disk_dir() is not None
+    except Exception:
+        return False

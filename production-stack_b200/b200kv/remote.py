@@ -5,29 +5,25 @@
 * `RemoteServer` / `python -m b200kv.server host port` — the server (C++ threads inside libb200kv.so;
   chunks live in a b200kv pool with the usual LRU).
 * `RemoteClient` — one connection (ctypes over the C ABI `b200kv_remote_*`).
-* `RemoteTier` — what the connector uses:
-    - scheduler role: `prefetch_state(req_id, tokens)` — when the local pool holds less than the whole
-      prompt, ask the server which further chunks it has and fetch them INTO THE LOCAL PINNED POOL on
-      a background thread; the connector answers vLLM "ask me again" (`(None, False)`,
-      KVConnectorBase_V1.get_num_new_matched_tokens, base.py:453-486) until that is done, then the
-      ordinary local lookup sees the chunks and the ordinary load path moves them to the GPU.
+* `RemoteTier` — what the connector uses, a `LowerTier` (b200kv/lower_tier.py):
+    - scheduler role: `prefetch_state(req_id, tokens)` — fetch the chunks the server holds beyond the local
+      pool's prefix INTO THE LOCAL PINNED POOL, while the connector answers vLLM "ask me again";
     - worker role: `push(keys)` — after a store, upload the new chunks in the background.
+    A server that fails is not asked again for `retry_s`.
 No byte of a chunk passes through Python: sockets <-> pool slots inside the library.
 """
 from __future__ import annotations
 
 import ctypes as C
 import logging
-import queue
 import threading
 import time
-from concurrent.futures import Future, ThreadPoolExecutor
 
 import numpy as np
 
-from . import _lib
 from ._lib import B200KVError, PoolStats, check, lib
-from .engine import KVPool, chunk_keys
+from .engine import KVPool
+from .lower_tier import LowerTier
 
 logger = logging.getLogger("b200kv")
 
@@ -126,36 +122,22 @@ class RemoteClient:
             pass
 
 
-class RemoteTier:
-    PENDING, DONE = "pending", "done"
+class RemoteTier(LowerTier):
+    name = "remote"
 
     def __init__(self, pool: KVPool, host: str, port: int, chunk: int, key_seed, owner: int = 0,
                  include_partial: bool = True, workers: int = 2, wait_s: float = 2.0, timeout_ms: int = 5000,
                  retry_s: float = 5.0, io_conns: int = 4):
         """key_seed: one seed, or one per tensor-parallel rank (the scheduler prefetches every rank's
-        chunks of a prompt; each worker pushes its own)."""
-        self.pool, self.host, self.port = pool, host, port
-        self.key_seeds = [int(x) for x in (key_seed if isinstance(key_seed, (list, tuple)) else [key_seed])]
-        self.chunk, self.owner, self.include_partial = chunk, owner, include_partial
-        self.wait_s, self.timeout_ms, self.retry_s = wait_s, timeout_ms, retry_s
+        chunks of a prompt; each worker pushes its own).  The chunk transfers of ONE prefetch run on
+        `io_conns` connections: one TCP stream is bounded by one core's copy rate, the rate scales with
+        connections."""
+        super().__init__(pool, chunk, key_seed, owner, include_partial, workers=workers, wait_s=wait_s,
+                         io_lanes=io_conns)
+        self.host, self.port = host, port
+        self.timeout_ms, self.retry_s = timeout_ms, retry_s
         self._tls = threading.local()
-        self._exec = ThreadPoolExecutor(max_workers=workers, thread_name_prefix="b200kv-remote")
-        # chunk transfers of ONE prefetch run on several connections (one TCP stream is bounded by one core's
-        # copy rate; the rate scales with connections)
-        self._io = ThreadPoolExecutor(max_workers=max(1, io_conns), thread_name_prefix="b200kv-remote-io")
-        self._io_conns = max(1, io_conns)
-        self._jobs: dict[str, tuple[Future, float]] = {}
-        self._asked: set[str] = set()                # requests whose one prefetch has been answered
         self._down_until = 0.0                       # server unreachable: do not stall requests on it
-        self._push_q: queue.Queue = queue.Queue()
-        self._pusher: threading.Thread | None = None
-        self._closed = False
-        self._inflight = 0                           # chunks queued or being uploaded
-        self._inflight_mu = threading.Lock()
-        self.fetched_chunks = 0
-        self.pushed_chunks = 0
-        self.push_skipped = 0
-        self.errors = 0
 
     # ---- connections (one per thread) -------------------------------------------------------------
     def _client(self) -> RemoteClient:
@@ -171,6 +153,10 @@ class RemoteTier:
             c.close()
             self._tls.client = None
 
+    # ---- LowerTier ----------------------------------------------------------------------------------
+    def _usable(self) -> bool:
+        return time.monotonic() >= self._down_until
+
     def _failed(self, what: str, err):
         self.errors += 1
         self._down_until = time.monotonic() + self.retry_s
@@ -178,128 +164,19 @@ class RemoteTier:
         logger.warning("b200kv remote tier %s:%d: %s failed (%s); local tier only for %.0f s",
                        self.host, self.port, what, err, self.retry_s)
 
-    # ---- scheduler role ---------------------------------------------------------------------------
-    def _get_some(self, keys) -> int:
-        c = self._client()
-        got = 0
-        for k in keys:
-            rc = c.get(self.pool, int(k), self.owner)
-            if rc == EIO:
-                self._drop_client()
-                raise B200KVError(rc, "b200kv_remote_get")
-            if rc != 0:              # evicted meanwhile / no local room: nothing behind it is useful
-                break
-            got += 1
-        return got
+    def _prefix(self, keys) -> int:
+        return self._client().exists(keys)
 
-    def _fetch(self, missing: list[np.ndarray]) -> int:
-        try:
-            c = self._client()
-            got = 0
-            for keys in missing:
-                n = c.exists(keys)
-                lanes = min(self._io_conns, n)
-                futs = [self._io.submit(self._get_some, keys[i:n:lanes]) for i in range(lanes)]
-                got += sum(f.result() for f in futs)
-            self.fetched_chunks += got
-            return got
-        except Exception as e:
-            self._failed("prefetch", e)
-            return 0
+    def _get(self, key: int) -> int:
+        rc = self._client().get(self.pool, key, self.owner)
+        if rc == EIO:
+            self._drop_client()
+            raise B200KVError(rc, "b200kv_remote_get")
+        return rc
 
-    def prefetch_state(self, req_id: str, tokens) -> str:
-        """PENDING while chunks of this prompt are on their way from the server, else DONE.
-        Never raises; a dead server degrades to the local tier."""
-        job = self._jobs.get(req_id)
-        now = time.monotonic()
-        if job is not None:
-            fut, t0 = job
-            if fut.done() or now - t0 > self.wait_s:
-                self._jobs.pop(req_id, None)      # late chunks still land in the pool for the next turn
-                self._asked.add(req_id)           # one prefetch per request, however often vLLM asks
-                return self.DONE
-            return self.PENDING
-        if self._closed or now < self._down_until or req_id in self._asked:
-            return self.DONE
-        missing = []
-        for seed in self.key_seeds:
-            keys = chunk_keys(tokens, self.chunk, seed, self.include_partial)
-            n_local = self.pool.lookup_owner(keys)[0] if len(keys) else 0
-            if n_local < len(keys):
-                missing.append(keys[n_local:].copy())
-        if not missing:
-            return self.DONE
-        self._jobs[req_id] = (self._exec.submit(self._fetch, missing), now)
-        return self.PENDING
-
-    def forget(self, req_id: str):
-        self._jobs.pop(req_id, None)
-        self._asked.discard(req_id)
-
-    # ---- worker role ------------------------------------------------------------------------------
-    def push(self, keys):
-        """Upload these chunks once they are READY in the local pool (the D2H of a store is still in
-        flight when this is called)."""
-        if self._closed:
-            return
-        if self._pusher is None:
-            self._pusher = threading.Thread(target=self._push_loop, name="b200kv-remote-push", daemon=True)
-            self._pusher.start()
-        keys = [int(k) for k in keys]
-        with self._inflight_mu:
-            self._inflight += len(keys)
-        for k in keys:
-            self._push_q.put((k, time.monotonic()))
-
-    def _settled(self):
-        with self._inflight_mu:
-            self._inflight -= 1
-
-    def _push_loop(self):
-        while True:
-            item = self._push_q.get()
-            if item is None:
-                return
-            key, t0 = item
-            if time.monotonic() < self._down_until:
-                self.push_skipped += 1
-                self._settled()
-                continue
-            try:
-                rc = self._client().put(self.pool, key, self.owner)
-                if rc == _lib.ENOENT and time.monotonic() - t0 < 10.0:
-                    time.sleep(0.002)                       # not committed yet: try again shortly
-                    self._push_q.put((key, t0))
-                    continue
-                if rc == 0:
-                    self.pushed_chunks += 1
-                elif rc in (_lib.ENOENT, _lib.EEXIST, _lib.ENOSPC):
-                    self.push_skipped += 1
-                else:
-                    raise B200KVError(rc, "b200kv_remote_put")
-            except Exception as e:
-                self._failed("push", e)
-            self._settled()
-
-    def flush(self, timeout_s: float = 30.0) -> bool:
-        """Wait until the push queue is drained (tests, shutdown)."""
-        t0 = time.monotonic()
-        while time.monotonic() - t0 < timeout_s:
-            with self._inflight_mu:
-                if self._inflight <= 0:
-                    return True
-            time.sleep(0.005)
-        return False
+    def _put(self, key: int) -> int:
+        return self._client().put(self.pool, key, self.owner)
 
     def stats(self) -> dict:
         return {"fetched_chunks": self.fetched_chunks, "pushed_chunks": self.pushed_chunks,
-                "push_skipped": self.push_skipped, "errors": self.errors}
-
-    def close(self):
-        self._closed = True
-        if self._pusher is not None:
-            self._push_q.put(None)
-            self._pusher.join(timeout=5)
-            self._pusher = None
-        self._exec.shutdown(wait=False, cancel_futures=True)
-        self._io.shutdown(wait=False, cancel_futures=True)
+                "push_skipped": self.push_skipped + self.push_present, "errors": self.errors}

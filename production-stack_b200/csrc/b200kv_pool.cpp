@@ -638,6 +638,52 @@ extern "C" int b200kv_pool_release(b200kv_pool* pool, uint64_t key) {
   return B200KV_OK;
 }
 
+extern "C" int b200kv_pool_place(b200kv_pool* pool, const uint32_t* slots, const uint64_t* keys,
+                                 const int32_t* n_tokens, const uint32_t* fmts, const uint32_t* owners, int32_t n) {
+  if (!pool || n < 0 || (n > 0 && (!slots || !keys || !n_tokens || !fmts || !owners))) return B200KV_EINVAL;
+  b200kv_pool::Guard g(pool);
+  int32_t placed = 0;
+  const uint64_t t = now_ns();
+  for (int32_t i = 0; i < n; ++i) {
+    const uint32_t s = slots[i];
+    if (s >= pool->h->n_slots || pool->slots[s].state != kFree || n_tokens[i] <= 0 || pool->find(keys[i]) != kNone)
+      continue;
+    Slot& e = pool->slots[s];
+    e.key = keys[i];
+    e.state = kReady;
+    e.fmt = fmts[i];
+    e.n_tokens = n_tokens[i];
+    e.owner = owners[i];
+    e.pins = 0;
+    e.lease_until_ns = 0;
+    e.touched_ns = t;
+    pool->table_insert(s);
+    pool->lru_push_tail(s);
+    ++pool->h->n_used;
+    ++placed;
+  }
+  if (placed) {  // the free list skips the slots just taken
+    pool->h->free_head = kNone;
+    for (uint32_t s = pool->h->n_slots; s-- > 0;) {
+      if (pool->slots[s].state != kFree) continue;
+      pool->slots[s].free_next = pool->h->free_head;
+      pool->h->free_head = s;
+    }
+  }
+  return placed;
+}
+
+extern "C" int b200kv_pool_drop(b200kv_pool* pool, uint64_t key) {
+  if (!pool) return B200KV_EINVAL;
+  b200kv_pool::Guard g(pool);
+  const uint32_t s = pool->find(key);
+  if (s == kNone || pool->slots[s].state != kReady) return B200KV_ENOENT;
+  if (pool->slots[s].pins) return B200KV_EBUSY;
+  pool->lru_unlink(s);
+  pool->free_slot(s);
+  return B200KV_OK;
+}
+
 extern "C" int b200kv_pool_get_stats(b200kv_pool* pool, b200kv_pool_stats* out) {
   if (!pool || !out) return B200KV_EINVAL;
   b200kv_pool::Guard g(pool);
