@@ -386,6 +386,29 @@ int b200kv_import_peer(b200kv_ctx* ctx, int32_t peer_id, int32_t peer_device,
 int b200kv_import_peer_ptrs(b200kv_ctx* ctx, int32_t peer_id, int32_t peer_device,
                             const void* const* k_ptrs, const void* const* v_ptrs,
                             uint64_t peer_block_stride_bytes, uint64_t peer_n_blocks);
+/* A peer replica of another tensor-parallel size (disaggregated prefill at one TP size, decode at another).  Its
+ * K/V planes hold peer_heads KV heads per token; heads [src_head0, src_head0 + n_heads) of them are this engine's
+ * heads [dst_head0, dst_head0 + n_heads).  Both sides keep the engine's block_tokens, head_dim, elem_bytes and tile
+ * order (NHD or HND).  Which slice a rank pulls from which peer rank: production-stack_b200/b200kv/pd.py, head_slices. */
+typedef struct b200kv_head_slice {
+  int32_t peer_heads;   /* H_p: KV heads per token in the peer's planes                              */
+  int32_t src_head0;    /* first head of the slice among the peer's                                  */
+  int32_t dst_head0;    /* first head of the slice among this engine's                               */
+  int32_t n_heads;      /* heads in the slice                                                        */
+} b200kv_head_slice;
+/* b200kv_import_peer / b200kv_import_peer_ptrs of a peer with a head slice: the peer is installed with its slice or
+ * not at all, and b200kv_peer_pull_async from it moves the slice's heads only (stats.p2p_bytes counts those).
+ * -EINVAL for a NULL slice, a slice outside [0, peer_heads) or outside [0, n_kv_heads), head_dim * elem_bytes not a
+ * multiple of 16, a peer block stride below block_tokens * peer_heads * head_dim * elem_bytes, or an MLA engine
+ * (a latent is the same on every rank: import the peer whole).                                  */
+int b200kv_import_peer_sliced(b200kv_ctx* ctx, int32_t peer_id, int32_t peer_device,
+                              const b200kv_ipc_desc* descs, int32_t n_descs,
+                              uint64_t peer_block_stride_bytes, uint64_t peer_n_blocks,
+                              const b200kv_head_slice* slice);
+int b200kv_import_peer_ptrs_sliced(b200kv_ctx* ctx, int32_t peer_id, int32_t peer_device,
+                                   const void* const* k_ptrs, const void* const* v_ptrs,
+                                   uint64_t peer_block_stride_bytes, uint64_t peer_n_blocks,
+                                   const b200kv_head_slice* slice);
 /* Consumer-side pull: token i is read from peer slot src_slots[i] and written to local slot
  * dst_slots[i]; in-kernel P2P loads, no staging, no NCCL.  `compute_stream` waits for it.  */
 int b200kv_peer_pull_async(b200kv_ctx* ctx, int32_t peer_id, const int64_t* src_slots,

@@ -72,6 +72,12 @@ class IpcDesc(C.Structure):
     _fields_ = [("handle", C.c_uint8 * 64), ("offset", C.c_uint64), ("alloc_bytes", C.c_uint64)]
 
 
+class HeadSlice(C.Structure):
+    """b200kv_head_slice: heads [src_head0, src_head0 + n_heads) of a peer with peer_heads heads per token are this
+    engine's heads [dst_head0, dst_head0 + n_heads)."""
+    _fields_ = [("peer_heads", C.c_int32), ("src_head0", C.c_int32), ("dst_head0", C.c_int32), ("n_heads", C.c_int32)]
+
+
 _P = C.c_void_p
 _U64P = C.POINTER(C.c_uint64)
 _I64P = C.POINTER(C.c_int64)
@@ -126,6 +132,10 @@ SIGNATURES = {
     "b200kv_export_ipc": (C.c_int, [_P, C.POINTER(IpcDesc), C.c_int32]),
     "b200kv_import_peer": (C.c_int, [_P, C.c_int32, C.c_int32, C.POINTER(IpcDesc), C.c_int32, C.c_uint64, C.c_uint64]),
     "b200kv_import_peer_ptrs": (C.c_int, [_P, C.c_int32, C.c_int32, C.POINTER(_P), C.POINTER(_P), C.c_uint64, C.c_uint64]),
+    "b200kv_import_peer_sliced": (C.c_int, [_P, C.c_int32, C.c_int32, C.POINTER(IpcDesc), C.c_int32, C.c_uint64,
+                                            C.c_uint64, C.POINTER(HeadSlice)]),
+    "b200kv_import_peer_ptrs_sliced": (C.c_int, [_P, C.c_int32, C.c_int32, C.POINTER(_P), C.POINTER(_P), C.c_uint64,
+                                                 C.c_uint64, C.POINTER(HeadSlice)]),
     "b200kv_peer_pull_async": (C.c_int, [_P, C.c_int32, _I64P, _I64P, C.c_int64, _P, _U64P]),
     "b200kv_gather_chunks": (C.c_int, [_P, _I64P, C.c_int64, _U64P, _P]),
     "b200kv_scatter_chunks": (C.c_int, [_P, _I64P, C.c_int64, _U64P, _P]),

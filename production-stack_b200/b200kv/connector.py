@@ -147,6 +147,13 @@ def draft_layers_of(vllm_config) -> int:
     return int(n)
 
 
+def total_kv_heads_of(model_config) -> int:
+    """The model's KV heads over all tensor-parallel ranks (ModelConfig.get_total_num_kv_heads); 0 for a config that
+    cannot tell, with which P/D pairs replicas of the same tensor-parallel size only."""
+    f = getattr(model_config, "get_total_num_kv_heads", None)
+    return int(f()) if f else 0
+
+
 def _log_once(msg: str):
     if msg not in _LOGGED:
         _LOGGED.add(msg)
@@ -230,6 +237,8 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
         pc = vllm_config.parallel_config
         self._model = str(vllm_config.model_config.model)
         self._world = pc.tensor_parallel_size
+        # the model's KV heads over all ranks and MLA-ness: P/D pairs replicas of different tensor-parallel sizes by them
+        self._total_kv_heads = total_kv_heads_of(vllm_config.model_config)
         self._pool_name = pool_name_for(vllm_config, self.cfg, geom.chunk_bytes)
         if role == KVConnectorRole.SCHEDULER:
             try:
@@ -258,7 +267,8 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
         self._sched_counters: tuple = (0, 0, 0)   # worker: last counters received from this engine's scheduler
         if role == KVConnectorRole.SCHEDULER:
             self._pd = PDScheduler(self._engine_id, self._block_size,
-                                   lease_s=float(self.cfg.extra.get("pd_lease_s", 120.0)), tp_size=self._world)
+                                   lease_s=float(self.cfg.extra.get("pd_lease_s", 120.0)), tp_size=self._world,
+                                   total_kv_heads=self._total_kv_heads, mla=geom.mla)
             seed = self._key_seed(0)
             lease = self.cfg.lookup_lease_ms
             chunk = self._chunk
@@ -437,8 +447,10 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
                 self._worker.on_stored = lambda keys: [h(keys) for h in hooks]
         try:
             tp_rank = self._tp_rank()
-            publish_ipc(self._engine_id, self._engine, t0.device.index or 0, tp_rank, self._world)   # peers may pull from us
-            self._pdw = PDWorker(self._engine, self._engine_id, self._block_size, rank=tp_rank, tp_size=self._world)
+            publish_ipc(self._engine_id, self._engine, t0.device.index or 0, tp_rank, self._world,
+                        total_kv_heads=self._total_kv_heads)   # peers may pull from us
+            self._pdw = PDWorker(self._engine, self._engine_id, self._block_size, rank=tp_rank, tp_size=self._world,
+                                 total_kv_heads=self._total_kv_heads)
         except Exception as e:  # e.g. VMM-allocated cache (sleep mode): P/D pull unavailable, offload still works
             logger.warning("b200kv: cannot publish CUDA-IPC descriptors (%s); peer pull disabled", e)
         if self.cfg.enable_controller and self.cfg.controller_pull_url and rank == 0:

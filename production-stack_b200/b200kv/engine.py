@@ -665,20 +665,29 @@ class KVEngine:
         return bytes(arr)
 
     def import_peer(self, peer_id: int, peer_device: int, descs: bytes,
-                    peer_block_stride: int | None = None, peer_n_blocks: int | None = None):
+                    peer_block_stride: int | None = None, peer_n_blocks: int | None = None, head_slice=None):
+        """Map a peer's cache (b200kv_import_peer).  head_slice = (peer_heads, src_head0, dst_head0, n_heads): a peer
+        of another tensor-parallel size, of which pulls move those heads only (b200kv_import_peer_sliced)."""
         n = self.geom.n_descs
         arr = (_lib.IpcDesc * n).from_buffer_copy(descs)
-        check(lib().b200kv_import_peer(self._h, peer_id, peer_device, arr, n,
-                                        peer_block_stride or self.geom.stride,
-                                        peer_n_blocks or self.geom.n_blocks), "b200kv_import_peer")
+        stride, nb = peer_block_stride or self.geom.stride, peer_n_blocks or self.geom.n_blocks
+        if head_slice is None:
+            check(lib().b200kv_import_peer(self._h, peer_id, peer_device, arr, n, stride, nb), "b200kv_import_peer")
+        else:
+            check(lib().b200kv_import_peer_sliced(self._h, peer_id, peer_device, arr, n, stride, nb,
+                                                   C.byref(_lib.HeadSlice(*head_slice))), "b200kv_import_peer_sliced")
 
     def import_peer_ptrs(self, peer_id: int, peer_device: int, k_ptrs, v_ptrs,
-                         peer_block_stride: int | None = None, peer_n_blocks: int | None = None):
+                         peer_block_stride: int | None = None, peer_n_blocks: int | None = None, head_slice=None):
         ka, va = self._plane_ptrs(k_ptrs, v_ptrs)
-        check(lib().b200kv_import_peer_ptrs(self._h, peer_id, peer_device, ka, va,
-                                             peer_block_stride or self.geom.stride,
-                                             peer_n_blocks or self.geom.n_blocks),
-              "b200kv_import_peer_ptrs")
+        stride, nb = peer_block_stride or self.geom.stride, peer_n_blocks or self.geom.n_blocks
+        if head_slice is None:
+            check(lib().b200kv_import_peer_ptrs(self._h, peer_id, peer_device, ka, va, stride, nb),
+                  "b200kv_import_peer_ptrs")
+        else:
+            check(lib().b200kv_import_peer_ptrs_sliced(self._h, peer_id, peer_device, ka, va, stride, nb,
+                                                        C.byref(_lib.HeadSlice(*head_slice))),
+                  "b200kv_import_peer_ptrs_sliced")
 
     def peer_pull(self, peer_id: int, src_slots, dst_slots, stream=None) -> int:
         s, d = _as_i64(src_slots), _as_i64(dst_slots)

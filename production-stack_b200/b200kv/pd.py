@@ -12,10 +12,19 @@ protocol is unchanged: route_orchestrated_disaggregated_request sends the prefil
 Here the decode replica reads the prefill replica's pages directly over NVSwitch
 (b200kv_peer_pull_async): no staging buffer, no UCX, no NCCL.  Control plane on one box:
   * every worker (one per tensor-parallel rank) publishes the CUDA-IPC descriptors of its paged cache
-    in /dev/shm/b200kv-ipc-<engine_id>.r<rank>.json (b200kv_export_ipc); decode rank r pulls from
-    prefill rank r, and the two sides must have the same tensor-parallel size (`tp_size` in the params);
+    in /dev/shm/b200kv-ipc-<engine_id>.r<rank>.json (b200kv_export_ipc), with the model's total KV-head count;
+    at the same tensor-parallel size (`tp_size` in the params) decode rank r pulls from prefill rank r;
+  * at different sizes each decode rank pulls its KV heads from the prefill ranks that hold them.  vLLM shards
+    T KV heads over t ranks (QKVParallelLinear): rank r holds H = max(1, T // t) heads, global heads
+    [r*H, (r+1)*H) when T >= t, else head r // (t / T), replicated t / T times.  For every local head the
+    first prefill rank holding it is the source; per (decode rank, prefill rank) pair that is one contiguous
+    head slice (head_slices), pulled by the head-slice kernel (b200kv_import_peer_sliced).  An MLA latent (and
+    V3.2's indexer plane) is the same on every rank: decode rank c pulls whole pages from prefill rank c % t_p;
   * the producer keeps a finished request's blocks (`delay_free=True`) until every consumer rank dropped
-    a marker /dev/shm/b200kv-done-<producer_engine_id>.r<rank>/<request_id>, or a lease expires;
+    a marker /dev/shm/b200kv-done-<producer_engine_id>.r<rank>/<request_id>, or a lease expires.  When
+    the sizes differ, decode rank c of t_d drops <request_id>.d<c>of<t_d> into the marker directory of EVERY
+    prefill rank, also of those it read nothing from, and a prefill rank releases the request once it holds
+    all t_d of them;
   * the LEASE is a file /dev/shm/b200kv-lease-<producer_engine_id>/<lease_id>, created by the producer's
     scheduler before it hands out the params and removed by it right before the blocks are freed
     (update_connector_output precedes the free, vllm/v1/core/sched/scheduler.py:2136-2165).  A consumer
@@ -27,15 +36,18 @@ from __future__ import annotations
 
 import base64
 import json
+import logging
 import os
+import re
 import time
 from dataclasses import dataclass, field
 
 import numpy as np
 
-from ._lib import DTYPE_BF16
+from ._lib import DTYPE_BF16, LAYOUT_MLA
 
 SHM_DIR = os.environ.get("B200KV_SHM_DIR", "/dev/shm")
+logger = logging.getLogger("b200kv")
 
 
 def _safe(s: str) -> str:
@@ -88,9 +100,12 @@ def _draft_of(geom) -> int:
     return int(getattr(geom, "draft_layers", 0))
 
 
-def publish_ipc(engine_id: str, engine, device: int, rank: int = 0, tp_size: int = 1) -> str:
+def publish_ipc(engine_id: str, engine, device: int, rank: int = 0, tp_size: int = 1, total_kv_heads: int = 0) -> str:
+    """total_kv_heads: the model's KV heads over all ranks (model_config.get_total_num_kv_heads()).  A document
+    without it pairs with consumers of its own tensor-parallel size only."""
     g = engine.geom
     doc = {"engine_id": engine_id, "device": device, "pid": os.getpid(), "rank": rank, "tp_size": tp_size,
+           **({"total_kv_heads": int(total_kv_heads)} if total_kv_heads else {}),
            "n_blocks": g.n_blocks,
            "block_stride": g.stride, "n_layers": g.n_layers, "n_kv_heads": g.n_kv_heads, "head_dim": g.head_dim,
            "block_tokens": g.block_tokens, "elem_bytes": g.elem_bytes, "layout": g.layout, "dtype": _dtype_of(g),
@@ -124,14 +139,120 @@ def unpublish_ipc(engine_id: str, rank: int = 0):
             pass
 
 
-class PeerResolver:
-    """remote engine_id -> peer_id of this engine; maps the peer's cache on first use."""
+# ------------------------------------------------------------------------------------------------
+# the head map of a pairing of different tensor-parallel sizes
+# ------------------------------------------------------------------------------------------------
+def shardable(total_kv_heads: int, tp_size: int) -> bool:
+    """vLLM can shard T KV heads over t ranks: t divides T, or T divides t (replication)."""
+    T, t = int(total_kv_heads), int(tp_size)
+    return T > 0 and t > 0 and (T % t == 0 if T >= t else t % T == 0)
 
-    def __init__(self, engine, max_peers: int = 64, rank: int = 0, tp_size: int = 1):
+
+def heads_of_rank(total_kv_heads: int, tp_size: int, rank: int) -> list[int]:
+    """Global KV heads that tensor-parallel rank `rank` of `tp_size` holds, in local order (QKVParallelLinear)."""
+    T, t = total_kv_heads, tp_size
+    if T >= t:
+        H = T // t
+        return list(range(rank * H, (rank + 1) * H))
+    return [rank // (t // T)]
+
+
+def head_slices(total_kv_heads: int, producer_tp: int, consumer_tp: int, consumer_rank: int):
+    """[(producer rank, (peer_heads, src_head0, dst_head0, n_heads))] for consumer rank `consumer_rank`, producer
+    ranks ascending: each local head is read from the first producer rank that holds it, and the heads read from one
+    producer rank are one contiguous slice on both sides.  ValueError if a size cannot shard the heads."""
+    T = int(total_kv_heads)
+    for t in (producer_tp, consumer_tp):
+        if not shardable(T, t):
+            raise ValueError(f"{T} KV heads cannot be sharded over {t} tensor-parallel ranks")
+    H_p = max(1, T // producer_tp)
+    by_rank: dict[int, list[tuple[int, int]]] = {}
+    for h, g in enumerate(heads_of_rank(T, consumer_tp, consumer_rank)):
+        p, src = (g // H_p, g % H_p) if T >= producer_tp else (g * (producer_tp // T), 0)
+        by_rank.setdefault(p, []).append((src, h))
+    out = []
+    for p in sorted(by_rank):
+        (src0, dst0), n = by_rank[p][0], len(by_rank[p])
+        if by_rank[p] != [(src0 + i, dst0 + i) for i in range(n)]:
+            raise ValueError(f"heads of producer rank {p} are not one contiguous slice: {by_rank[p]}")
+        out.append((p, (H_p, src0, dst0, n)))
+    return out
+
+
+class PeerResolver:
+    """remote engine_id -> peer_id of this engine; maps the peer's cache on first use.  A remote engine of another
+    tensor-parallel size maps as one peer per producer rank this rank reads from (sources)."""
+
+    def __init__(self, engine, max_peers: int = 64, rank: int = 0, tp_size: int = 1, total_kv_heads: int = 0):
         self.engine = engine
-        self.ids: dict[str, int] = {}
+        self.ids: dict = {}     # remote engine_id (same size), or (engine_id, producer rank) -> peer_id
         self.max_peers = max_peers
         self.rank, self.tp_size = rank, tp_size
+        self.total_kv_heads = int(total_kv_heads)
+        self._sources: dict[str, list] = {}
+
+    def sources(self, remote_engine_id: str, remote_tp_size: int) -> list[tuple[int, tuple | None]]:
+        """[(peer_id, head slice or None)] to pull from for a request prefilled by `remote_engine_id` at tensor-parallel
+        size `remote_tp_size`: [(resolve(), None)] at this rank's size; else one source per producer rank read."""
+        if remote_tp_size == self.tp_size:
+            return [(self.resolve(remote_engine_id), None)]
+        src = self._sources.get(remote_engine_id)
+        if src is not None:
+            return src
+        g = self.engine.geom
+        if getattr(g, "layout", 0) == LAYOUT_MLA:
+            pairs = [(self.rank % remote_tp_size, None)]     # the latent is the same on every rank
+        elif not self.total_kv_heads:
+            raise ValueError(f"peer {remote_engine_id}: tensor-parallel size {remote_tp_size} differs from local "
+                             f"{self.tp_size} and the local total KV-head count is not known")
+        elif g.n_kv_heads != max(1, self.total_kv_heads // self.tp_size):
+            raise ValueError(f"local cache holds {g.n_kv_heads} KV heads, {self.total_kv_heads} heads over "
+                             f"{self.tp_size} ranks imply {max(1, self.total_kv_heads // self.tp_size)}")
+        else:
+            pairs = head_slices(self.total_kv_heads, remote_tp_size, self.tp_size, self.rank)
+        src = []
+        for p, sl in pairs:
+            pid = self.ids.get((remote_engine_id, p))
+            if pid is None:
+                doc = self._doc(remote_engine_id, p, remote_tp_size)
+                if sl is None:
+                    self._check(remote_engine_id, doc, "n_kv_heads", g.n_kv_heads)
+                else:
+                    if int(doc.get("total_kv_heads", 0)) != self.total_kv_heads:
+                        raise ValueError(f"peer {remote_engine_id}.r{p}: total_kv_heads={doc.get('total_kv_heads')} "
+                                         f"differs from local {self.total_kv_heads} (a replica that does not publish it "
+                                         "pairs at its own tensor-parallel size only)")
+                    self._check(remote_engine_id, doc, "n_kv_heads", sl[0])   # the head map's per-rank count
+                pid = self._import((remote_engine_id, p), doc, sl)
+            src.append((pid, sl))
+        self._sources[remote_engine_id] = src
+        logger.info("b200kv P/D: engine %s at tensor-parallel size %d pairs with local rank %d of %d: %s",
+                    remote_engine_id, remote_tp_size, self.rank, self.tp_size,
+                    ", ".join(f"rank {p} " + ("whole pages" if sl is None else
+                                              f"heads [{sl[1]}, {sl[1] + sl[3]}) -> [{sl[2]}, {sl[2] + sl[3]})")
+                              for p, sl in pairs))
+        return src
+
+    def _doc(self, remote_engine_id: str, rank: int, tp_size: int) -> dict:
+        with open(ipc_path(remote_engine_id, rank)) as f:
+            doc = json.load(f)
+        if int(doc.get("tp_size", 1)) != tp_size or int(doc.get("rank", 0)) != rank:
+            raise ValueError(f"peer {remote_engine_id}: tensor-parallel layout {doc.get('rank')}/{doc.get('tp_size')} "
+                             f"differs from the expected {rank}/{tp_size}")
+        return doc
+
+    def _import(self, key, doc: dict, head_slice) -> int:
+        pid = len(self.ids)
+        if pid >= self.max_peers:
+            raise RuntimeError("too many peers")
+        descs = base64.b64decode(doc["descs"])
+        if head_slice is None:
+            self.engine.import_peer(pid, doc["device"], descs, doc["block_stride"], doc["n_blocks"])
+        else:
+            self.engine.import_peer(pid, doc["device"], descs, doc["block_stride"], doc["n_blocks"],
+                                    head_slice=head_slice)
+        self.ids[key] = pid
+        return pid
 
     def resolve(self, remote_engine_id: str) -> int:
         pid = self.ids.get(remote_engine_id)
@@ -142,6 +263,11 @@ class PeerResolver:
         if int(doc.get("tp_size", 1)) != self.tp_size or int(doc.get("rank", 0)) != self.rank:
             raise ValueError(f"peer {remote_engine_id}: tensor-parallel layout {doc.get('rank')}/{doc.get('tp_size')} "
                              f"differs from local {self.rank}/{self.tp_size}")
+        self._check(remote_engine_id, doc, "n_kv_heads", self.engine.geom.n_kv_heads)
+        return self._import(remote_engine_id, doc, None)
+
+    def _check(self, remote_engine_id: str, doc: dict, heads_key: str, heads: int):
+        """The peer's cache has this engine's geometry; heads_key names the head count compared."""
         g = self.engine.geom
         doc.setdefault("dtype", DTYPE_BF16)   # documents published before the field are bf16 caches
         doc.setdefault("indexer", 0)          # ... and caches without indexer planes
@@ -152,17 +278,11 @@ class PeerResolver:
             raise ValueError(f"peer {remote_engine_id}: n_layers={doc['n_layers']} with {doc['draft_layers']} draft "
                              f"layer(s) differs from local {g.n_layers} with {_draft_of(g)}: replicas pair only "
                              "with the same speculative-decoding drafter, or both without one")
-        for k, mine in (("n_kv_heads", g.n_kv_heads), ("head_dim", g.head_dim),
+        for k, mine in ((heads_key, heads), ("head_dim", g.head_dim),
                         ("block_tokens", g.block_tokens), ("elem_bytes", g.elem_bytes), ("layout", g.layout),
                         ("dtype", _dtype_of(g)), ("indexer", _indexer_of(g))):
             if doc[k] != mine:
                 raise ValueError(f"peer {remote_engine_id}: {k}={doc[k]} differs from local {mine}")
-        pid = len(self.ids)
-        if pid >= self.max_peers:
-            raise RuntimeError("too many peers")
-        self.engine.import_peer(pid, doc["device"], base64.b64decode(doc["descs"]), doc["block_stride"], doc["n_blocks"])
-        self.ids[remote_engine_id] = pid
-        return pid
 
 
 def slots_of(block_ids, block_tokens: int, n_tokens: int) -> np.ndarray:
@@ -183,6 +303,7 @@ class PullSpec:
     n_tokens: int          # tokens [skip_tokens, n_tokens) are pulled
     skip_tokens: int = 0   # already computed locally (block aligned): left untouched
     remote_lease_id: str = ""   # the producer's lease on its blocks (checked before and after the pull)
+    remote_tp_size: int = 0     # the producer's tensor-parallel size (`tp_size` in the params); 0: the consumer's
 
 
 @dataclass
@@ -194,11 +315,14 @@ class PDMeta:
 
 class PDScheduler:
     def __init__(self, engine_id: str, block_size: int, lease_s: float = 120.0, tp_size: int = 1,
-                 blocks_known_at_alloc: bool = True):
+                 blocks_known_at_alloc: bool = True, total_kv_heads: int = 0, mla: bool = False):
         self.engine_id = engine_id
         self.block_size = block_size
         self.lease_s = lease_s
         self.tp_size = tp_size
+        # the model's head geometry: with it, a producer of another tensor-parallel size is paired (module docstring);
+        # without it such a request is declined
+        self.total_kv_heads, self.mla = int(total_kv_heads), bool(mla)
         # False under vLLM's LMCacheConnectorV1 wrapper, which drops `blocks` from update_state_after_alloc
         # (lmcache_connector.py:253-262): a pull would have nowhere to land, so remote prefills are declined
         # there and the request is served by the pool lookup / recomputed
@@ -215,13 +339,21 @@ class PDScheduler:
         p = getattr(request, "kv_transfer_params", None)
         if not p or not p.get("do_remote_prefill") or not p.get("remote_block_ids") or not p.get("remote_engine_id"):
             return None
-        if not self.blocks_known_at_alloc or int(p.get("tp_size") or 1) != self.tp_size:
-            return None      # cannot pull (see __init__ / different tensor-parallel layout): ordinary request
+        if not self.blocks_known_at_alloc or not self.pairs_with(int(p.get("tp_size") or 1)):
+            return None      # cannot pull (see __init__ / unpairable tensor-parallel layout): ordinary request
         n_prompt = len(request.prompt_token_ids or [])
         n_remote = min(int(p.get("remote_num_tokens") or n_prompt), n_prompt,
                        len(first_group(p["remote_block_ids"])) * self.block_size)
         # the last prompt token is recomputed locally (same rule as a full pool hit)
         return max(min(n_remote, n_prompt - 1) - num_computed_tokens, 0)
+
+    def pairs_with(self, remote_tp_size: int) -> bool:
+        """A producer at tensor-parallel size remote_tp_size can hand its KV to this consumer."""
+        if remote_tp_size == self.tp_size:
+            return True
+        if self.mla:
+            return remote_tp_size > 0
+        return shardable(self.total_kv_heads, remote_tp_size) and shardable(self.total_kv_heads, self.tp_size)
 
     def after_alloc(self, request, local_block_ids: list[int], num_external_tokens: int, num_computed_tokens: int = 0):
         p = getattr(request, "kv_transfer_params", None)
@@ -237,7 +369,7 @@ class PDScheduler:
             remote_block_ids=first_group(p["remote_block_ids"]), local_block_ids=list(local_block_ids),
             n_tokens=num_computed_tokens + num_external_tokens,
             skip_tokens=num_computed_tokens // self.block_size * self.block_size,
-            remote_lease_id=str(p.get("remote_lease_id") or ""))
+            remote_lease_id=str(p.get("remote_lease_id") or ""), remote_tp_size=int(p.get("tp_size") or 1))
 
     # ---- producer -------------------------------------------------------------------------
     def request_finished(self, request, block_ids: list[int], finished_ok: bool = True):
@@ -292,6 +424,29 @@ class PDScheduler:
             pass
 
 
+_SPLIT = re.compile(r"(.+)\.d(\d+)of(\d+)")
+
+
+def split_marker(request_id: str, consumer_rank: int, consumer_tp: int) -> str:
+    """Marker of consumer rank `consumer_rank` of `consumer_tp` in a pairing of different tensor-parallel sizes."""
+    return f"{_safe(request_id)}.d{int(consumer_rank)}of{int(consumer_tp)}"
+
+
+def split_markers(names) -> dict[str, dict[int, set[int]]]:
+    """Marker file names -> {request id: {consumer tp size: consumer ranks that dropped a marker}}."""
+    out: dict[str, dict[int, set[int]]] = {}
+    for name in names:
+        m = _SPLIT.fullmatch(name)
+        if m and int(m.group(2)) < int(m.group(3)):
+            out.setdefault(m.group(1), {}).setdefault(int(m.group(3)), set()).add(int(m.group(2)))
+    return out
+
+
+def released(ranks_by_tp: dict[int, set[int]]) -> bool:
+    """Every consumer rank of some tensor-parallel size has dropped its marker."""
+    return any(len(cs) == n for n, cs in ranks_by_tp.items())
+
+
 def first_group(block_ids):
     if block_ids and isinstance(block_ids[0], (list, tuple)):
         return list(block_ids[0])
@@ -302,13 +457,14 @@ def first_group(block_ids):
 # worker-role state
 # ------------------------------------------------------------------------------------------------
 class PDWorker:
-    def __init__(self, engine, engine_id: str, block_size: int, resolver=None, rank: int = 0, tp_size: int = 1):
+    def __init__(self, engine, engine_id: str, block_size: int, resolver=None, rank: int = 0, tp_size: int = 1,
+                 total_kv_heads: int = 0):
         self.engine = engine
         self.engine_id = engine_id
         self.block_size = block_size
-        self.rank = rank
-        self.resolver = resolver or PeerResolver(engine, rank=rank, tp_size=tp_size)
-        self._inflight: list[tuple[int, PullSpec]] = []   # (ticket, spec)
+        self.rank, self.tp_size = rank, tp_size
+        self.resolver = resolver or PeerResolver(engine, rank=rank, tp_size=tp_size, total_kv_heads=total_kv_heads)
+        self._inflight: list[tuple[list[int], PullSpec]] = []   # (tickets, spec): one pull per source
         self._held: dict[str, float] = {}
         self.failed_blocks: set[int] = set()
         self.n_pulled_tokens = 0
@@ -318,9 +474,15 @@ class PDWorker:
     def _lease_alive(spec: PullSpec) -> bool:
         return not spec.remote_lease_id or os.path.exists(lease_path(spec.remote_engine_id, spec.remote_lease_id))
 
+    def _mismatched(self, spec: PullSpec) -> bool:
+        return bool(spec.remote_tp_size) and spec.remote_tp_size != self.tp_size
+
     def start_pulls(self, meta: PDMeta, stream=None):
+        """One pull per source of each request, on `stream`.  The lease is checked before the first and (poll) after
+        the last; a request any of whose pulls cannot be issued has all its local blocks reported."""
         self._held.update(meta.held)
         for spec in meta.pulls:
+            tickets: list[int] = []
             try:
                 n = min(spec.n_tokens, len(spec.remote_block_ids) * self.block_size)
                 if len(spec.local_block_ids) * self.block_size < n:
@@ -329,30 +491,41 @@ class PDWorker:
                 if not self._lease_alive(spec):
                     self.n_lease_failures += 1
                     raise TimeoutError("the producer's lease on the blocks has expired")
-                peer = self.resolver.resolve(spec.remote_engine_id)
+                if self._mismatched(spec):
+                    peers = [pid for pid, _ in self.resolver.sources(spec.remote_engine_id, spec.remote_tp_size)]
+                else:
+                    peers = [self.resolver.resolve(spec.remote_engine_id)]
                 src = slots_of(spec.remote_block_ids, self.block_size, n)[spec.skip_tokens:]
                 dst = slots_of(spec.local_block_ids, self.block_size, n)[spec.skip_tokens:]
                 if len(src) == 0:
                     self._notify_done(spec)
                     continue
                 trace("pull_issued", req=spec.req_id, tokens=int(len(src)), rank=self.rank)
-                ticket = self.engine.peer_pull(peer, src, dst, stream=stream)
-                self._inflight.append((ticket, spec))
+                for peer in peers:
+                    tickets.append(self.engine.peer_pull(peer, src, dst, stream=stream))
+                self._inflight.append((tickets, spec))
                 self.n_pulled_tokens += len(src)
             except Exception as e:
                 # no exception on the data path: vLLM recomputes the blocks we report
                 trace("pull_failed", req=spec.req_id, error=repr(e), rank=self.rank)
+                for t in tickets:      # pulls already issued read the producer's pages until they finish
+                    self.engine.wait(t)
                 self.failed_blocks.update(spec.local_block_ids)
                 self._notify_done(spec)
 
     def _notify_done(self, spec: PullSpec):
-        d = done_dir(spec.remote_engine_id, self.rank)
-        try:
-            os.makedirs(d, exist_ok=True)
-            with open(os.path.join(d, _safe(spec.remote_request_id)), "w"):
-                pass
-        except OSError:
-            pass  # the producer's lease will expire instead
+        if self._mismatched(spec):    # every producer rank waits for every consumer rank
+            marks = [(done_dir(spec.remote_engine_id, p), split_marker(spec.remote_request_id, self.rank, self.tp_size))
+                     for p in range(spec.remote_tp_size)]
+        else:
+            marks = [(done_dir(spec.remote_engine_id, self.rank), _safe(spec.remote_request_id))]
+        for d, name in marks:
+            try:
+                os.makedirs(d, exist_ok=True)
+                with open(os.path.join(d, name), "w"):
+                    pass
+            except OSError:
+                pass  # the producer's lease will expire instead
 
     def poll(self, block: bool = False) -> tuple[set[str], set[str]]:
         """-> (finished_sending, finished_recving) request ids for get_finished().  block=True (what the
@@ -360,10 +533,11 @@ class PDWorker:
         costs the pull itself — so that a pull invalidated by an expired lease is reported as load errors in
         the SAME step (get_block_ids_with_load_errors follows get_finished)."""
         recv_done, still = set(), []
-        for ticket, spec in self._inflight:
+        for tickets, spec in self._inflight:
             if block:
-                self.engine.wait(ticket)
-            if block or self.engine.poll(ticket):
+                for t in tickets:
+                    self.engine.wait(t)
+            if block or all(self.engine.poll(t) for t in tickets):
                 if not self._lease_alive(spec):     # freed (and maybe recycled) while we were reading
                     self.n_lease_failures += 1
                     self.failed_blocks.update(spec.local_block_ids)
@@ -373,7 +547,7 @@ class PDWorker:
                 self._notify_done(spec)
                 recv_done.add(spec.req_id)
             else:
-                still.append((ticket, spec))
+                still.append((tickets, spec))
         self._inflight = still
         send_done = set()
         if self._held:
@@ -382,15 +556,18 @@ class PDWorker:
                 marks = set(os.listdir(d))
             except OSError:
                 marks = set()
+            split = split_markers(marks)
             now = time.monotonic()
             for rid, deadline in list(self._held.items()):
-                if _safe(rid) in marks or now > deadline:
+                sid = _safe(rid)
+                if sid in marks or released(split.get(sid, {})) or now > deadline:
                     send_done.add(rid)
                     self._held.pop(rid)
-                    try:
-                        os.unlink(os.path.join(d, _safe(rid)))     # this rank's own marker directory
-                    except OSError:
-                        pass
+                    for name in [sid] + [split_marker(rid, c, n) for n, cs in split.get(sid, {}).items() for c in cs]:
+                        try:
+                            os.unlink(os.path.join(d, name))     # this rank's own marker directory
+                        except OSError:
+                            pass
         return send_done, recv_done
 
     def take_failed_blocks(self) -> set[int]:

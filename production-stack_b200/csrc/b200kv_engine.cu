@@ -136,6 +136,10 @@ struct Peer {
   uint64_t block_stride = 0;
   uint64_t n_blocks = 0;
   std::vector<void*> opened;  // cudaIpcOpenMemHandle mappings to close
+  // a peer of another tensor-parallel size (b200kv_import_peer_sliced): its planes hold slice.peer_heads heads per
+  // token, and a pull moves slice.n_heads of them; pulls from it take kv_head_slice_pull_kernel
+  bool sliced = false;
+  b200kv_head_slice slice{};
 };
 
 struct Geometry {
@@ -637,8 +641,26 @@ int launch_indexer(b200kv_ctx* ctx, CopyMode mode, const TableView& tv, size_t f
 int launch_planes(b200kv_ctx* ctx, CopyMode mode, const OpTable& t, const TableView& tv, uint32_t c0, uint32_t c1,
                   cudaStream_t s, uint32_t pb, uint32_t np, const Peer* peer);
 
+// A pull from a sliced peer: every run of the table (full, then partial) through kv_head_slice_pull_kernel, the
+// slice in the KernelArgs fields the kernel names.  Sliced peers exist on K/V engines only, so there are no
+// indexer planes.
+int launch_slice_pull(b200kv_ctx* ctx, const OpTable& t, const TableView& tv, cudaStream_t s, const Peer& peer) {
+  const Geometry& g = ctx->g;
+  KernelArgs a = kernel_args(ctx, tv, 0, 0, 0, &peer);
+  a.peer.token_bytes = static_cast<uint32_t>(peer.slice.peer_heads) * g.row_bytes;
+  a.chunk.chunk_tokens = static_cast<uint32_t>(peer.slice.n_heads);
+  a.chunk.slab_bytes = static_cast<uint64_t>(peer.slice.src_head0);
+  a.chunk.scales_off = static_cast<uint64_t>(peer.slice.dst_head0);
+  a.total_units = static_cast<uint32_t>(t.runs.size()) * a.n_planes;
+  const uint32_t grid = std::min<uint32_t>(a.total_units, static_cast<uint32_t>(ctx->sm_count) * 8u);
+  if (grid == 0) return B200KV_OK;
+  kv_head_slice_pull_kernel<<<grid, kSliceThreads, 0, s>>>(a);
+  return launched(ctx);
+}
+
 int launch_op(b200kv_ctx* ctx, CopyMode mode, const OpTable& t, const TableView& tv, uint32_t c0, uint32_t c1,
               cudaStream_t s, uint32_t pb = 0, uint32_t np = 0, const Peer* peer = nullptr) {
+  if (peer && peer->sliced) return launch_slice_pull(ctx, t, tv, s, *peer);
   const int rc = launch_planes(ctx, mode, t, tv, c0, c1, s, pb, np, peer);
   if (rc || !ctx->g.indexed) return rc;
   const size_t f0 = t.full_off[c0], nf = t.full_off[c1] - f0;   // MLA tables have full runs only
@@ -1705,12 +1727,30 @@ extern "C" int b200kv_export_ipc(b200kv_ctx* ctx, b200kv_ipc_desc* descs_out, in
   return B200KV_OK;
 }
 
-// Installs a peer whole or not at all: ctx->peers[peer_id] is written only once its base table is on the device.
-// It then owns `opened`; on failure nothing of the peer is left, and the caller still owns `opened`.
+// A head slice a K/V engine can pull (b200kv_import_peer_sliced): inside [0, peer_heads) and [0, H), whole 16-byte
+// rows, and a peer block stride that holds a block of peer_heads heads.
+static int check_slice(const Geometry& g, const b200kv_head_slice& sl, uint64_t peer_block_stride) {
+  if (g.mla || g.row_bytes % 16) return B200KV_EINVAL;
+  if (sl.peer_heads <= 0 || sl.peer_heads > 65536 || sl.n_heads <= 0 || sl.src_head0 < 0 || sl.dst_head0 < 0 ||
+      sl.src_head0 + sl.n_heads > sl.peer_heads || sl.dst_head0 + sl.n_heads > static_cast<int32_t>(g.H))
+    return B200KV_EINVAL;
+  if (peer_block_stride < static_cast<uint64_t>(g.bs) * static_cast<uint64_t>(sl.peer_heads) * g.row_bytes)
+    return B200KV_EINVAL;
+  return B200KV_OK;
+}
+
+// Installs a peer whole or not at all: ctx->peers[peer_id] is written only once its base table is on the device,
+// with its head slice when `slice` is given.  It then owns `opened`; on failure nothing of the peer is left, and the
+// caller still owns `opened`.
 static int install_peer(b200kv_ctx* ctx, int32_t peer_id, int32_t peer_device, const std::vector<uint64_t>& bases,
-                        uint64_t stride, uint64_t n_blocks, std::vector<void*>* opened) {
+                        uint64_t stride, uint64_t n_blocks, std::vector<void*>* opened,
+                        const b200kv_head_slice* slice) {
   if (ctx->peers[peer_id].valid) return B200KV_EEXIST;
   Peer p;
+  if (slice) {
+    p.sliced = true;
+    p.slice = *slice;
+  }
   CU_TRY(cudaMalloc(&p.d_bases, sizeof(uint64_t) * bases.size()));
   const cudaError_t e = cudaMemcpy(p.d_bases, bases.data(), sizeof(uint64_t) * bases.size(), cudaMemcpyHostToDevice);
   if (e != cudaSuccess) {
@@ -1727,13 +1767,14 @@ static int install_peer(b200kv_ctx* ctx, int32_t peer_id, int32_t peer_device, c
   return B200KV_OK;
 }
 
-extern "C" int b200kv_import_peer(b200kv_ctx* ctx, int32_t peer_id, int32_t peer_device,
-                                  const b200kv_ipc_desc* descs, int32_t n_descs,
-                                  uint64_t peer_block_stride_bytes, uint64_t peer_n_blocks) {
+static int import_peer(b200kv_ctx* ctx, int32_t peer_id, int32_t peer_device, const b200kv_ipc_desc* descs,
+                       int32_t n_descs, uint64_t peer_block_stride_bytes, uint64_t peer_n_blocks,
+                       const b200kv_head_slice* slice) {
   if (!ctx || !descs || peer_id < 0 || peer_id >= kMaxPeers) return B200KV_EINVAL;
   const Geometry& g = ctx->g;
   if (n_descs != static_cast<int32_t>(g.n_bases) || peer_n_blocks == 0 || peer_n_blocks * g.bs > 0x7fffffffull)
     return B200KV_EINVAL;
+  if (slice && check_slice(g, *slice, peer_block_stride_bytes)) return B200KV_EINVAL;
   DeviceGuard dg(ctx->cfg.device);
   std::lock_guard<std::mutex> lk(ctx->mu);
   // one cudaIpcOpenMemHandle per distinct allocation
@@ -1761,17 +1802,33 @@ extern "C" int b200kv_import_peer(b200kv_ctx* ctx, int32_t peer_id, int32_t peer
     }
     bases[base_slot(g, i / g.L, i % g.L)] = reinterpret_cast<uint64_t>(base) + d.offset;
   }
-  if (rc == B200KV_OK) rc = install_peer(ctx, peer_id, peer_device, bases, peer_block_stride_bytes, peer_n_blocks, &opened);
+  if (rc == B200KV_OK)
+    rc = install_peer(ctx, peer_id, peer_device, bases, peer_block_stride_bytes, peer_n_blocks, &opened, slice);
   if (rc)   // the mappings this call opened; install_peer took none of them
     for (void* m : opened) cudaIpcCloseMemHandle(m);
   return rc;
 }
 
-extern "C" int b200kv_import_peer_ptrs(b200kv_ctx* ctx, int32_t peer_id, int32_t peer_device,
-                                       const void* const* k_ptrs, const void* const* v_ptrs,
-                                       uint64_t peer_block_stride_bytes, uint64_t peer_n_blocks) {
+extern "C" int b200kv_import_peer(b200kv_ctx* ctx, int32_t peer_id, int32_t peer_device,
+                                  const b200kv_ipc_desc* descs, int32_t n_descs,
+                                  uint64_t peer_block_stride_bytes, uint64_t peer_n_blocks) {
+  return import_peer(ctx, peer_id, peer_device, descs, n_descs, peer_block_stride_bytes, peer_n_blocks, nullptr);
+}
+
+extern "C" int b200kv_import_peer_sliced(b200kv_ctx* ctx, int32_t peer_id, int32_t peer_device,
+                                         const b200kv_ipc_desc* descs, int32_t n_descs,
+                                         uint64_t peer_block_stride_bytes, uint64_t peer_n_blocks,
+                                         const b200kv_head_slice* slice) {
+  if (!slice) return B200KV_EINVAL;
+  return import_peer(ctx, peer_id, peer_device, descs, n_descs, peer_block_stride_bytes, peer_n_blocks, slice);
+}
+
+static int import_peer_ptrs(b200kv_ctx* ctx, int32_t peer_id, int32_t peer_device, const void* const* k_ptrs,
+                            const void* const* v_ptrs, uint64_t peer_block_stride_bytes, uint64_t peer_n_blocks,
+                            const b200kv_head_slice* slice) {
   if (!ctx || peer_id < 0 || peer_id >= kMaxPeers) return B200KV_EINVAL;
   if (peer_n_blocks == 0 || peer_n_blocks * ctx->g.bs > 0x7fffffffull) return B200KV_EINVAL;
+  if (slice && check_slice(ctx->g, *slice, peer_block_stride_bytes)) return B200KV_EINVAL;
   DeviceGuard dg(ctx->cfg.device);
   std::lock_guard<std::mutex> lk(ctx->mu);
   std::vector<uint64_t> bases;
@@ -1789,7 +1846,21 @@ extern "C" int b200kv_import_peer_ptrs(b200kv_ctx* ctx, int32_t peer_id, int32_t
     cudaGetLastError();
   }
   std::vector<void*> none;   // raw pointers: no mappings to close
-  return install_peer(ctx, peer_id, peer_device, bases, peer_block_stride_bytes, peer_n_blocks, &none);
+  return install_peer(ctx, peer_id, peer_device, bases, peer_block_stride_bytes, peer_n_blocks, &none, slice);
+}
+
+extern "C" int b200kv_import_peer_ptrs(b200kv_ctx* ctx, int32_t peer_id, int32_t peer_device,
+                                       const void* const* k_ptrs, const void* const* v_ptrs,
+                                       uint64_t peer_block_stride_bytes, uint64_t peer_n_blocks) {
+  return import_peer_ptrs(ctx, peer_id, peer_device, k_ptrs, v_ptrs, peer_block_stride_bytes, peer_n_blocks, nullptr);
+}
+
+extern "C" int b200kv_import_peer_ptrs_sliced(b200kv_ctx* ctx, int32_t peer_id, int32_t peer_device,
+                                              const void* const* k_ptrs, const void* const* v_ptrs,
+                                              uint64_t peer_block_stride_bytes, uint64_t peer_n_blocks,
+                                              const b200kv_head_slice* slice) {
+  if (!slice) return B200KV_EINVAL;
+  return import_peer_ptrs(ctx, peer_id, peer_device, k_ptrs, v_ptrs, peer_block_stride_bytes, peer_n_blocks, slice);
 }
 
 extern "C" int b200kv_peer_pull_async(b200kv_ctx* ctx, int32_t peer_id, const int64_t* src_slots,
@@ -1843,7 +1914,9 @@ extern "C" int b200kv_peer_pull_async(b200kv_ctx* ctx, int32_t peer_id, const in
   if (!detached) CU_TRY(cudaStreamWaitEvent(cs, op->done, 0));
   ++ctx->stats.n_pull_ops;
   ctx->stats.n_pulled_tokens += n_tokens;
-  ctx->stats.p2p_bytes += static_cast<uint64_t>(n_tokens) * ctx->g.token_bytes * ctx->g.planes;
+  const uint64_t token_bytes = peer.sliced ? static_cast<uint64_t>(peer.slice.n_heads) * ctx->g.row_bytes
+                                           : ctx->g.token_bytes;
+  ctx->stats.p2p_bytes += static_cast<uint64_t>(n_tokens) * token_bytes * ctx->g.planes;
   if (ctx->g.indexed) ctx->stats.p2p_bytes += static_cast<uint64_t>(n_tokens) * (ctx->g.idx_vb + ctx->g.idx_sb) * ctx->g.L;
   *ticket = op->id;
   ctx->ops.emplace(op->id, std::move(guard.op));

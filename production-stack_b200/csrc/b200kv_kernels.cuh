@@ -33,6 +33,8 @@
 //   kv_mla_fp8_load_kernel     128 elements is 16 lanes; no shared memory.
 //   kv_indexer_copy_kernel the indexer planes of sparse-attention MLA engines (split [values][scales] tiles),
 //                          verbatim, store / load / pull: TMA bulk pieces, a 4-byte warp copy for unaligned scales.
+//   kv_head_slice_pull_kernel  peer pull from a replica of another tensor-parallel size: a contiguous range of the
+//                          peer's heads into a contiguous range of ours, 16-byte vectors.
 //
 // Every kernel takes one KernelArgs, filled by kernel_args() in b200kv_engine.cu.  The seven FP8 / Q4 / MLA FP8
 // kernels are also built per cache element type (bf16, fp16: template argument DT, see Src below).
@@ -1211,6 +1213,71 @@ __global__ void __launch_bounds__(kIdxWarps * 32) kv_indexer_copy_kernel(const K
     }
   }
   if (lane == 0) bulk_wait_all<0>();   // every store has landed before the grid is considered complete
+}
+
+// ---------------------------------------------------------------------------------------------
+// Head-slice peer pull: a producer replica of another tensor-parallel size holds heads [src_head0, src_head0 + n)
+// of its H_p local heads that this engine keeps at [dst_head0, dst_head0 + n) of its H (b200kv_import_peer_sliced).
+// K/V planes only.  Runs come from build_pull_runs (run.a = peer slot, run.b = local slot, never across a block).
+// A pull reads no chunk, so KernelArgs carry the slice in the chunk side's fields:
+//   peer.token_bytes   H_p * D * elem    (the peer's NHD token row)
+//   paged.token_bytes  H * D * elem      (ours)
+//   chunk.chunk_tokens n: heads moved
+//   chunk.slab_bytes   src_head0: first head of the slice among the peer's
+//   chunk.scales_off   dst_head0: where it lands among ours
+//   row_bytes          D * elem (a multiple of 16)
+// A unit is one (run, plane), total_units = n_runs * n_planes, and moves `cnt` pieces of `len` bytes:
+//   NHD  cnt = run.n rows of n * D * elem, strided by each side's token row
+//   HND  a whole-block run is one piece of n * bs * D * elem (the slice's tiles are adjacent on both sides);
+//        a partial run is n pieces of run.n * D * elem, one per head, strided by bs * D * elem
+// The CTA copies the unit's 16-byte vectors (flattened over pieces) with ld.global.nc from the peer mapping, read
+// over NVLink as in kv_bulk_copy_kernel<kPull>, four in flight per thread.  No shared memory, no barrier.
+// ---------------------------------------------------------------------------------------------
+constexpr int kSliceThreads = 256;
+
+__global__ void __launch_bounds__(kSliceThreads) kv_head_slice_pull_kernel(const KernelArgs p) {
+  const uint32_t bs = p.paged.block_tokens, row = p.row_bytes, nh = p.chunk.chunk_tokens;
+  for (uint32_t u = blockIdx.x; u < p.total_units; u += gridDim.x) {
+    const uint32_t plane = p.plane_begin + u % p.n_planes;
+    const Run run = p.runs[u / p.n_planes];
+    const uint32_t sb = static_cast<uint32_t>(run.a) / bs, so = static_cast<uint32_t>(run.a) - sb * bs;
+    const uint32_t db = static_cast<uint32_t>(run.b) / bs, dof = static_cast<uint32_t>(run.b) - db * bs;
+    const uint8_t* src = reinterpret_cast<const uint8_t*>(__ldg(p.peer.bases + plane) +
+                                                          static_cast<uint64_t>(sb) * p.peer.block_stride);
+    uint8_t* dst = reinterpret_cast<uint8_t*>(__ldg(p.paged.bases + plane) +
+                                              static_cast<uint64_t>(db) * p.paged.block_stride);
+    uint32_t cnt, len, ss, ds;
+    if (!p.hnd) {
+      src += static_cast<uint64_t>(so) * p.peer.token_bytes + p.chunk.slab_bytes * row;
+      dst += static_cast<uint64_t>(dof) * p.paged.token_bytes + p.chunk.scales_off * row;
+      cnt = static_cast<uint32_t>(run.n);
+      len = nh * row;
+      ss = p.peer.token_bytes;
+      ds = p.paged.token_bytes;
+    } else {
+      const uint32_t tile = bs * row;
+      src += p.chunk.slab_bytes * tile + static_cast<uint64_t>(so) * row;
+      dst += p.chunk.scales_off * tile + static_cast<uint64_t>(dof) * row;
+      const bool whole = static_cast<uint32_t>(run.n) == bs;
+      cnt = whole ? 1u : nh;
+      len = whole ? nh * tile : static_cast<uint32_t>(run.n) * row;
+      ss = ds = tile;
+    }
+    const uint32_t vpp = len >> 4, nvec = cnt * vpp;
+    auto at = [&](uint32_t i, uint32_t stride) {
+      const uint32_t k = i / vpp;
+      return static_cast<uint64_t>(k) * stride + static_cast<uint64_t>(i - k * vpp) * 16u;
+    };
+    uint32_t i = threadIdx.x;
+    for (; i + 3 * kSliceThreads < nvec; i += 4 * kSliceThreads) {
+      uint4 v[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) v[j] = ld_nc_v4(src + at(i + j * kSliceThreads, ss));
+#pragma unroll
+      for (int j = 0; j < 4; ++j) st_na_v4(dst + at(i + j * kSliceThreads, ds), v[j]);
+    }
+    for (; i < nvec; i += kSliceThreads) st_na_v4(dst + at(i, ds), ld_nc_v4(src + at(i, ss)));
+  }
 }
 
 }  // namespace b200kv
