@@ -61,16 +61,22 @@ extern "C" {
 #define B200KV_FMT_FP8 1
 /* Q4 (experimental): group-wise 4-bit — per (token, head) groups of 32 elements, bf16 scale = absmax/7,
  * two's-complement nibbles; a stored token of one plane is [H*D/2 codes][H*D/32 scales] (4.5 bits per
- * element).  Specified by oracle/kv_oracle.py q4_pack_chunk (tests/fp16_oracle.py for fp16 caches).
- * Source dtype bf16 or fp16 (the scales stay bf16 for both), D % 32 == 0.                         */
+ * element).  Specified by oracle/kv_oracle.py q4_pack_chunk (tests/fp16_oracle.py for fp16 caches,
+ * tests/fp8_cache_oracle.py for fp8 caches).  Source dtype bf16, fp16, e4m3 or e5m2 (the scales stay bf16 for
+ * all), D % 32 == 0; on fp8 caches also H*D % 64 == 0.                                            */
 #define B200KV_FMT_Q4 2
 
 /* ---- element type of the paged cache (b200kv_set_cache_dtype) ---------------------------- */
-/* The lossy formats decode the cache's 16-bit elements, so they must know which type they are.  RAW moves
+/* The lossy formats decode the cache's elements, so they must know which type they are.  RAW moves
  * bytes and needs no type, but the type is part of every chunk's format tag in either case, so bf16 and
- * fp16 chunks never mix in a pool, a device tier or a cache server.                          */
+ * fp16 chunks, and e4m3 and e5m2 chunks, never mix in a pool, a device tier or a cache server.
+ * On a 1-byte (fp8) engine the default type 0 means e4m3 (vLLM's fp8 / fp8_e4m3 caches, e4m3fn): fp8 engines
+ * created before the fp8 types existed were e4m3 in practice and keep their tags.  Q4 is the one lossy format
+ * of an fp8 cache (tests/fp8_cache_oracle.py); FP8 is refused there, the pages already are fp8.          */
 #define B200KV_DTYPE_BF16 0   /* default */
 #define B200KV_DTYPE_FP16 1
+#define B200KV_DTYPE_E4M3 0   /* the default of a 1-byte engine: the same value as BF16, so the same tags */
+#define B200KV_DTYPE_E5M2 2
 
 /* ---- order inside one (block, K|V) tile of the paged cache ------------------------------ */
 /* NHD: [block_tokens][H][D] (FlashAttention default, vllm/v1/attention/backends/flash_attn.py:
@@ -261,8 +267,9 @@ typedef struct b200kv_engine_stats {
 /* Engine construction (stands in for _init_lmcache_engine, vllm_v1_adapter.py:433-558).
  * `pool` may be NULL for an engine used only through gather/scatter/peer_pull.             */
 int b200kv_engine_create(const b200kv_engine_config* cfg, b200kv_pool* pool, b200kv_ctx** out);
-/* Element type of the cache, B200KV_DTYPE_* (bf16 until set).  Legal between b200kv_engine_create and
- * b200kv_register_kv: -EBUSY after registration.  FP16 needs elem_bytes == 2, else -EINVAL.  A function
+/* Element type of the cache, B200KV_DTYPE_* (bf16, or e4m3 on a 1-byte engine, until set).  Legal between
+ * b200kv_engine_create and b200kv_register_kv: -EBUSY after registration.  FP16 needs elem_bytes == 2 and E5M2
+ * elem_bytes == 1, else -EINVAL.  A function
  * rather than a config field, so the v1 config layout and every existing binding stay valid.     */
 int b200kv_set_cache_dtype(b200kv_ctx* ctx, int32_t dtype);
 /* Gives an MLA engine an indexer plane per layer (B200KV_LAYOUT_MLA, indexer planes above); block_stride_bytes is

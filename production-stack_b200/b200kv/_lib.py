@@ -16,6 +16,7 @@ FMT_RAW, FMT_FP8, FMT_Q4 = 0, 1, 2   # FMT_Q4: experimental (group-wise 4-bit)
 VARIANT_BULK, VARIANT_LDG = 0, 1
 LAYOUT_NHD, LAYOUT_HND, LAYOUT_MLA = 0, 1, 2   # LAYOUT_MLA: one latent plane per layer (DeepSeek-V2/V3, Kimi-K2)
 DTYPE_BF16, DTYPE_FP16 = 0, 1                  # element type of the cache (b200kv_set_cache_dtype)
+DTYPE_E4M3, DTYPE_E5M2 = 0, 2                  # ... of a 1-byte (fp8) cache: e4m3 is the default, value 0 as bf16
 FMT_TAG_INDEXED = 1 << 24                      # format-tag bit of chunks with indexer planes (b200kv_set_indexer)
 POOL_CREATE, POOL_ATTACH, POOL_CREATE_OR_ATTACH = 1, 2, 3
 NUMA_LOCAL, NUMA_INTERLEAVE, NUMA_OFF = 0, 1, 2

@@ -25,8 +25,8 @@ from vllm.distributed.kv_transfer.kv_connector.v1.base import (KVConnectorBase_V
 from . import _lib
 from .adapter import ReqMeta, SchedulerState, WorkerState, request_identity
 from .config import B200KVConfig
-from .engine import (INDEXER_SCALE_BYTES, INDEXER_VALUE_BYTES, KVEngine, KVGeometry, KVPool, dtype_code,
-                     paged_layout_of, split_indexer_caches, xxh64)
+from .engine import (FP8_CACHE_DTYPES, INDEXER_SCALE_BYTES, INDEXER_VALUE_BYTES, KVEngine, KVGeometry, KVPool,
+                     dtype_code, paged_layout_of, split_indexer_caches, xxh64)
 from .pd import PDMeta, PDScheduler, PDWorker, first_group, publish_ipc, unpublish_ipc
 
 if TYPE_CHECKING:
@@ -77,7 +77,10 @@ def geometry_from_vllm(vllm_config, cfg: B200KVConfig, n_blocks: int = 1) -> KVG
     (vllm_v1_adapter.py:471-477), derivable in both roles from the vLLM config alone.  An MLA model
     (model_config.use_mla) has one latent plane per layer: (num_layer, 1, chunk, 1, head_size)
     (vllm_v1_adapter.py:463-477).  The cache's element type: the model's with cache_dtype "auto",
-    named by "float16" / "bfloat16"; every other cache dtype (fp8*, ...) keeps bf16, which only RAW reads.
+    named by "float16" / "bfloat16".  Of a 1-byte cache, dtype stays bf16 and fp8_dtype says which fp8 type it holds:
+    "fp8" and "fp8_e4m3" are e4m3 and "fp8_e5m2" is e5m2 (FP8_CACHE_DTYPES).  On
+    those fp8 caches Q4 quantises the codes, and FP8 is stored RAW: the pages already are fp8.  Every other 1-byte
+    cache dtype (fp8_per_token_head, fp8_inc) keeps the default type, which only RAW reads, and Q4 is refused.
     An MLA model with DeepSeek Sparse Attention (DeepSeek-V3.2: index_topk in the HF config, vLLM's test) also
     has an indexer key cache per layer, which the geometry's indexer planes describe.  With the fp8_ds_mla cache a
     latent token is already a 656-byte FP8 record, so the chunk stores it RAW, also when FP8 is asked for.
@@ -101,6 +104,13 @@ def geometry_from_vllm(vllm_config, cfg: B200KVConfig, n_blocks: int = 1) -> KVG
         if fmt == _lib.FMT_FP8:
             fmt = _lib.FMT_RAW
             _log_once("b200kv: the fp8_ds_mla cache already holds FP8 latent records: chunks are stored RAW")
+    elif dt in FP8_CACHE_DTYPES and fmt == _lib.FMT_FP8:
+        fmt = _lib.FMT_RAW
+        _log_once(f"b200kv: the {dt} KV cache already holds fp8 codes, which the FP8 format would store as the same "
+                  "bytes: chunks are stored RAW")
+    elif elem == 1 and fmt == _lib.FMT_Q4 and dt not in FP8_CACHE_DTYPES:
+        raise ValueError(f"B200KV_FORMAT=q4 cannot read --kv-cache-dtype {dt}: Q4 takes bf16, fp16, fp8 (fp8_e4m3) "
+                         "and fp8_e5m2 caches; use B200KV_FORMAT=raw with this cache")
     hf = getattr(mc, "hf_text_config", None) or getattr(mc, "hf_config", None)
     sparse = mla and hasattr(hf, "index_topk")   # vLLM's own test for a V3.2 model (deepseek_v2.py, is_v32)
     draft = draft_layers_of(vllm_config)
@@ -109,6 +119,7 @@ def geometry_from_vllm(vllm_config, cfg: B200KVConfig, n_blocks: int = 1) -> KVG
                       head_dim=head_dim, n_blocks=n_blocks, block_tokens=cc.block_size,
                       chunk_tokens=cfg.chunk_size, elem_bytes=elem, block_stride_bytes=0, fmt=fmt,
                       layout=_lib.LAYOUT_MLA if mla else _lib.LAYOUT_NHD, dtype=dtype,
+                      fp8_dtype=FP8_CACHE_DTYPES.get(dt, _lib.DTYPE_E4M3),
                       idx_value_bytes=INDEXER_VALUE_BYTES if sparse else 0,
                       idx_scale_bytes=INDEXER_SCALE_BYTES if sparse else 0)
 
@@ -385,10 +396,17 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
                 raise ValueError(f"KV cache tensors do not match the model geometry: the speculative config implies "
                                  f"{D} draft layer(s) with indices {L}..{L + D - 1} after the {L} target layers, the "
                                  f"registered layers have {len(drafts)} at or above index {L}: {drafts}")
+        cache_dtype = str(self._vllm_config.cache_config.cache_dtype)
+        if t0.element_size() != geom0.elem_bytes:
+            raise ValueError(f"KV cache tensors hold {t0.element_size()}-byte elements ({t0.dtype}); the vLLM config's "
+                             f"cache dtype {cache_dtype!r} implies {geom0.elem_bytes}-byte ones")
+        # the tensor's type where it names one; vLLM's uint8 fp8 caches take the flavour the config names
+        code, fp8 = dtype_code(t0.dtype, cache_dtype), t0.element_size() == 1
         geom = KVGeometry(n_layers=len(tensors), n_kv_heads=h, head_dim=d, n_blocks=nb,
                           block_tokens=self._block_size, chunk_tokens=self._chunk,
                           elem_bytes=t0.element_size(), block_stride_bytes=stride, fmt=geom0.fmt,
-                          layout=tile_layout, dtype=dtype_code(t0.dtype) or _lib.DTYPE_BF16,
+                          layout=tile_layout, dtype=_lib.DTYPE_BF16 if fp8 else (code or _lib.DTYPE_BF16),
+                          fp8_dtype=(geom0.fp8_dtype if code is None else code) if fp8 else _lib.DTYPE_E4M3,
                           idx_value_bytes=INDEXER_VALUE_BYTES if idx else 0,
                           idx_scale_bytes=INDEXER_SCALE_BYTES if idx else 0,
                           idx_block_stride_bytes=idx[0].stride(0) if idx else 0,
@@ -400,7 +418,7 @@ class B200KVConnector(KVConnectorBase_V1, SupportsHMA):
             raise ValueError("KV cache tensors do not match the model geometry the pool was sized for "
                              f"({geom.chunk_bytes} vs {geom0.chunk_bytes} bytes per chunk, {len(tensors)} vs "
                              f"{geom0.n_layers} layers of which {geom0.draft_layers} draft layers)")
-        if geom.dtype != geom0.dtype:   # the key seed is derived from the vLLM config's type
+        if geom.cache_dtype != geom0.cache_dtype:   # the key seed is derived from the vLLM config's type
             raise ValueError(f"KV cache dtype {t0.dtype} differs from the one the vLLM config implies")
         rank = getattr(self._vllm_config.parallel_config, "rank", 0)
         self._rank = rank

@@ -63,10 +63,19 @@ def xxh64(data: bytes, seed: int = 0) -> int:
                                   C.c_uint64(seed)))
 
 
-def dtype_code(torch_dtype) -> int | None:
-    """torch dtype of a cache -> DTYPE_BF16 / DTYPE_FP16; None for every other type."""
+# vLLM's 1-byte cache dtypes whose codes the Q4 kernels decode (vLLM allocates them as torch.uint8)
+FP8_CACHE_DTYPES = {"fp8": _lib.DTYPE_E4M3, "fp8_e4m3": _lib.DTYPE_E4M3, "fp8_e5m2": _lib.DTYPE_E5M2}
+
+
+def dtype_code(torch_dtype, cache_dtype: str | None = None) -> int | None:
+    """torch dtype of a cache -> DTYPE_BF16 / DTYPE_FP16 / DTYPE_E4M3 / DTYPE_E5M2; None for every other type.
+    vLLM allocates fp8 caches as torch.uint8, so for a uint8 tensor the fp8 flavour comes from vLLM's
+    cache_config.cache_dtype (FP8_CACHE_DTYPES); without one, or for another 1-byte cache dtype, it is None."""
     name = str(torch_dtype)
-    return {"torch.bfloat16": _lib.DTYPE_BF16, "torch.float16": _lib.DTYPE_FP16}.get(name)
+    if name == "torch.uint8":
+        return FP8_CACHE_DTYPES.get(str(cache_dtype)) if cache_dtype is not None else None
+    return {"torch.bfloat16": _lib.DTYPE_BF16, "torch.float16": _lib.DTYPE_FP16,
+            "torch.float8_e4m3fn": _lib.DTYPE_E4M3, "torch.float8_e5m2": _lib.DTYPE_E5M2}.get(name)
 
 
 @dataclass(frozen=True)
@@ -92,6 +101,9 @@ class KVGeometry:
     # speculative decoding (MTP, EAGLE, EAGLE-3): how many of the n_layers are the drafter's, which vLLM puts in the
     # target's KV-cache group.  They are layers n_layers - draft_layers .. n_layers - 1, with the target's geometry.
     draft_layers: int = 0
+    # fp8 type of a 1-byte cache (vLLM's --kv-cache-dtype fp8 / fp8_e4m3 / fp8_e5m2): DTYPE_E4M3 (the default, the
+    # same value as DTYPE_BF16) or DTYPE_E5M2 (b200kv_set_cache_dtype)
+    fp8_dtype: int = _lib.DTYPE_E4M3
 
     def __post_init__(self):
         if not 0 <= self.draft_layers < max(self.n_layers, 1):
@@ -107,11 +119,27 @@ class KVGeometry:
         return self.dtype == _lib.DTYPE_FP16
 
     @property
+    def cache_dtype(self) -> int:
+        """The element type the engine holds (b200kv_set_cache_dtype) and records in format tags and P/D documents:
+        dtype on a 16-bit cache, fp8_dtype on a 1-byte one."""
+        return self.fp8_dtype if self.elem_bytes == 1 and self.dtype == _lib.DTYPE_BF16 else self.dtype
+
+    @property
+    def e5m2(self) -> bool:
+        return self.elem_bytes == 1 and self.cache_dtype == _lib.DTYPE_E5M2
+
+    @property
+    def dtype_name(self) -> str:
+        if self.elem_bytes == 1:
+            return "float8_e5m2" if self.e5m2 else "float8_e4m3fn"
+        return "float16" if self.fp16 else "bfloat16"
+
+    @property
     def fmt_tag(self) -> int:
         """The format tag the engine records with every chunk (pool_fmt in b200kv_engine.cu): format, tile order
         and cache element type, plus bit 24 with indexer planes.  bf16 tags are format | layout << 8, as before the
         element type was added."""
-        return self.fmt | (self.layout << 8) | (self.dtype << 16) | (_lib.FMT_TAG_INDEXED if self.indexed else 0)
+        return self.fmt | (self.layout << 8) | (self.cache_dtype << 16) | (_lib.FMT_TAG_INDEXED if self.indexed else 0)
 
     @property
     def token_bytes(self) -> int:
@@ -153,7 +181,8 @@ class KVGeometry:
         worker_id, ...) — chunks of different models / shards / formats never alias.  An MLA latent is
         the same on every tensor-parallel rank, so its namespace keeps only the pipeline stage
         (rank // world_size) of the rank: one stored copy serves every rank of the stage.  An fp16 cache
-        appends "|fp16", so its chunks (RAW included) never alias a bf16 replica's; bf16 seeds are unchanged.  A
+        appends "|fp16", so its chunks (RAW included) never alias a bf16 replica's; bf16 seeds are unchanged.  An
+        e5m2 cache appends "|e5m2" likewise, and e4m3 seeds are unchanged.  A
         geometry with indexer planes appends "|idx<bytes per token>" (V3.2: "|idx132"); others are unchanged.
         Draft layers count in n_layers, so a speculative-decoding replica's chunks, which carry the drafter's planes,
         have a namespace of their own; a geometry without draft layers keeps its seed."""
@@ -163,6 +192,8 @@ class KVGeometry:
               f"{self.elem_bytes}|{self.chunk_tokens}|{self.fmt}|{self.layout}"
         if self.fp16:
             tag += "|fp16"
+        if self.e5m2:
+            tag += "|e5m2"
         if self.indexed:
             tag += f"|idx{self.idx_token_bytes}"
         return xxh64(tag.encode(), DEFAULT_SEED)
@@ -424,8 +455,10 @@ class KVEngine:
               "b200kv_engine_create")
         self._h = h
         self._kv_refs = None
-        if geom.fp16:
-            self.set_cache_dtype(_lib.DTYPE_FP16)
+        if geom.dtype != _lib.DTYPE_BF16:
+            self.set_cache_dtype(geom.dtype)
+        if geom.fp8_dtype != _lib.DTYPE_E4M3:
+            self.set_cache_dtype(geom.fp8_dtype)    # -EINVAL unless the cache is 1-byte
         if geom.indexed:
             self.set_indexer(geom.idx_value_bytes, geom.idx_scale_bytes, geom.idx_stride)
 
@@ -479,11 +512,13 @@ class KVEngine:
                     or nb < self.geom.n_blocks or t.element_size() != self.geom.elem_bytes \
                     or tl != self.geom.layout:
                 raise ValueError("KV cache tensor does not match the engine geometry")
-            if self.geom.fmt != FMT_RAW and dtype_code(t.dtype) != self.geom.dtype:
+            code = dtype_code(t.dtype)
+            if self.geom.fmt != FMT_RAW and code != self.geom.cache_dtype and not (code is None and str(t.dtype) == "torch.uint8"):
                 # the lossy kernels decode the elements: fp16 bits read as bf16 (or the reverse) would be stored
-                # and loaded as wrong values without any error
+                # and loaded as wrong values without any error.  A uint8 tensor (how vLLM allocates fp8 caches)
+                # does not say which fp8 type it holds: the geometry does.
                 raise ValueError(f"KV cache dtype {t.dtype} does not match the engine's cache dtype "
-                                 f"({'float16' if self.geom.fp16 else 'bfloat16'})")
+                                 f"({self.geom.dtype_name})")
             k_ptrs.append(k)
             if not self.geom.mla:
                 v_ptrs.append(v)

@@ -86,8 +86,9 @@ def trace(event: str, **kw):
 # publication of a replica's cache (worker role, after register_kv_caches)
 # ------------------------------------------------------------------------------------------------
 def _dtype_of(geom) -> int:
-    """The cache element type of a geometry (KVGeometry.dtype; bf16 for a geometry without one)."""
-    return int(getattr(geom, "dtype", DTYPE_BF16))
+    """The cache element type of a geometry (KVGeometry.cache_dtype, else its dtype; bf16 for a geometry without
+    either)."""
+    return int(getattr(geom, "cache_dtype", getattr(geom, "dtype", DTYPE_BF16)))
 
 
 def _indexer_of(geom) -> int:
@@ -269,7 +270,7 @@ class PeerResolver:
     def _check(self, remote_engine_id: str, doc: dict, heads_key: str, heads: int):
         """The peer's cache has this engine's geometry; heads_key names the head count compared."""
         g = self.engine.geom
-        doc.setdefault("dtype", DTYPE_BF16)   # documents published before the field are bf16 caches
+        doc.setdefault("dtype", DTYPE_BF16)   # documents published before the field are bf16 caches (e4m3 on 1-byte ones)
         doc.setdefault("indexer", 0)          # ... and caches without indexer planes
         doc.setdefault("draft_layers", 0)     # ... and replicas without a speculative-decoding drafter
         if (doc["n_layers"], doc["draft_layers"]) != (g.n_layers, _draft_of(g)):

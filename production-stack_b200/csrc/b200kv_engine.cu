@@ -217,8 +217,9 @@ int make_geometry(const b200kv_engine_config* c, Geometry* g) {
     g->scales_bytes = static_cast<uint64_t>(g->planes) * g->H * sizeof(float);
     g->chunk_bytes = (g->scales_off + g->scales_bytes + 255) / 256 * 256;
   } else if (c->format == B200KV_FMT_Q4) {
-    if (g->elem != 2 || g->mla) return B200KV_ENOTSUP;
+    if ((g->elem != 2 && g->elem != 1) || g->mla) return B200KV_ENOTSUP;   // 16-bit or fp8 pages
     if (g->D % 32) return B200KV_EINVAL;
+    if (g->elem == 1 && (g->H * g->D) % 64) return B200KV_EINVAL;   // fp8 kernels: records 4-byte aligned
     g->fmt_token_bytes = g->H * g->D / 2 + g->H * (g->D / 32) * 2;   // one token record of one plane
     g->slab_bytes = static_cast<uint64_t>(g->C) * g->fmt_token_bytes;
     g->scales_off = 0;
@@ -585,6 +586,19 @@ size_t indexer_smem_bytes(const Geometry& g) {
   return kIdxBarBytes + static_cast<size_t>(kIdxWarps) * ((static_cast<size_t>(g.bs) * (g.idx_vb + g.idx_sb) + 15) & ~15ull);
 }
 
+// Q4 store or load of fp8 pages, runs [f0, f0 + nf): one unit per (run, plane), as launch_per_run.
+template <__nv_fp8_interpretation_t FT>
+int launch_q4_fp8(b200kv_ctx* ctx, CopyMode mode, const TableView& tv, size_t f0, size_t nf, cudaStream_t s,
+                  uint32_t plane_begin, uint32_t n_planes) {
+  KernelArgs a = kernel_args(ctx, tv, f0, plane_begin, n_planes);
+  a.total_units = static_cast<uint32_t>(nf) * a.n_planes;
+  const uint32_t grid = std::min<uint32_t>(a.total_units, static_cast<uint32_t>(ctx->sm_count) * 8u);
+  if (grid == 0) return B200KV_OK;
+  if (mode == kStore) kv_q4_store_fp8_kernel<FT><<<grid, 256, 0, s>>>(a);
+  else kv_q4_load_fp8_kernel<FT><<<grid, 256, 0, s>>>(a);
+  return launched(ctx);
+}
+
 // FP8 latent records of an MLA engine, either direction, runs [f0, f0 + nf): one warp per (run, plane) unit.
 template <int DT>
 int launch_mla_fp8(b200kv_ctx* ctx, CopyMode mode, const TableView& tv, size_t f0, size_t nf, cudaStream_t s,
@@ -673,6 +687,9 @@ int launch_planes(b200kv_ctx* ctx, CopyMode mode, const OpTable& t, const TableV
                   cudaStream_t s, uint32_t pb, uint32_t np, const Peer* peer) {
   const size_t f0 = t.full_off[c0], nf = t.full_off[c1] - f0;
   const int fmt = mode == kPull ? B200KV_FMT_RAW : ctx->cfg.format;
+  if (fmt != B200KV_FMT_RAW && ctx->g.elem == 1)   // Q4, the one lossy format of fp8 pages (make_geometry)
+    return ctx->g.dtype == B200KV_DTYPE_E5M2 ? launch_q4_fp8<__NV_E5M2>(ctx, mode, tv, f0, nf, s, pb, np)
+                                             : launch_q4_fp8<__NV_E4M3>(ctx, mode, tv, f0, nf, s, pb, np);
   if (fmt != B200KV_FMT_RAW)
     return ctx->g.dtype == B200KV_DTYPE_FP16 ? launch_lossy<kFp16>(ctx, mode, t, tv, f0, nf, s, pb, np)
                                              : launch_lossy<kBf16>(ctx, mode, t, tv, f0, nf, s, pb, np);
@@ -1144,10 +1161,12 @@ static void build_tensor_maps(b200kv_ctx* ctx, const std::vector<uint64_t>& base
 }
 
 extern "C" int b200kv_set_cache_dtype(b200kv_ctx* ctx, int32_t dtype) {
-  if (!ctx || (dtype != B200KV_DTYPE_BF16 && dtype != B200KV_DTYPE_FP16)) return B200KV_EINVAL;
+  if (!ctx || (dtype != B200KV_DTYPE_BF16 && dtype != B200KV_DTYPE_FP16 && dtype != B200KV_DTYPE_E5M2))
+    return B200KV_EINVAL;
   std::lock_guard<std::mutex> lk(ctx->mu);
   if (ctx->kv_registered) return B200KV_EBUSY;   // chunks already stored or moved under the old type
   if (dtype == B200KV_DTYPE_FP16 && ctx->g.elem != 2) return B200KV_EINVAL;
+  if (dtype == B200KV_DTYPE_E5M2 && ctx->g.elem != 1) return B200KV_EINVAL;
   ctx->g.dtype = static_cast<uint32_t>(dtype);
   return B200KV_OK;
 }
@@ -1187,6 +1206,10 @@ extern "C" int b200kv_register_kv(b200kv_ctx* ctx, const void* const* k_ptrs,
   if (!ctx) return B200KV_EINVAL;
   DeviceGuard dg(ctx->cfg.device);
   std::lock_guard<std::mutex> lk(ctx->mu);
+  // the Q4 kernels of fp8 pages decode e4m3 or e5m2 codes: no other type may reach them
+  if (ctx->cfg.format == B200KV_FMT_Q4 && ctx->g.elem == 1 && ctx->g.dtype != B200KV_DTYPE_E4M3 &&
+      ctx->g.dtype != B200KV_DTYPE_E5M2)
+    return B200KV_EINVAL;
   std::vector<uint64_t> h;
   const int rc = plane_bases(ctx->g, k_ptrs, v_ptrs, &h);
   if (rc) return rc;

@@ -29,6 +29,8 @@
 //   kv_fp8_load_kernel     bulk-load e4m3 piece -> dequantise -> 16-byte stores into the pages.
 //   kv_q4_store_kernel /   group-wise 4-bit chunks: one 16-byte vector per thread, a group is a quad
 //   kv_q4_load_kernel      of lanes.
+//   kv_q4_store_fp8_kernel /  the same records from and to fp8 pages (e4m3 or e5m2): a group is a pair of lanes.
+//   kv_q4_load_fp8_kernel
 //   kv_mla_fp8_store_kernel /  FP8 latent records of MLA engines: one warp per (token, plane), a group of
 //   kv_mla_fp8_load_kernel     128 elements is 16 lanes; no shared memory.
 //   kv_indexer_copy_kernel the indexer planes of sparse-attention MLA engines (split [values][scales] tiles),
@@ -80,7 +82,7 @@ struct KernelArgs {
   uint32_t pieces;                // bulk copy: pieces per run = ceil(block_tokens / piece_tokens)
   uint32_t piece_tokens;          // bulk copy: tokens per piece (piece bytes <= stage bytes)
   uint32_t total_units;           // units of work of the launch; each kernel says what its unit is
-  uint32_t row_bytes;             // D * elem: one (token, head) row (D*2 for FP8 / Q4, which take 16-bit caches only)
+  uint32_t row_bytes;             // D * elem: one (token, head) row (D*2 for FP8, D*2 or D for Q4)
   uint32_t hnd;                   // pages hold [H][block_tokens][D] tiles
 };
 static_assert(sizeof(KernelArgs) <= 128, "KernelArgs must stay within 128 bytes (see above)");
@@ -1025,6 +1027,146 @@ __global__ void __launch_bounds__(256) kv_q4_load_kernel(const KernelArgs p) {
           const int b = static_cast<int>((packed[j] >> (8 * i)) & 0xffu);
           const int ql = ((b & 0xF) ^ 8) - 8, qh = ((b >> 4) ^ 8) - 8;   // sign-extend the nibbles
           o[i] = Src<DT>::pack_rn(static_cast<float>(ql) * s, static_cast<float>(qh) * s);
+        }
+        st_na_v4(reinterpret_cast<void*>(q4_src_addr(p, plane, static_cast<uint32_t>(run.a) + tt[j], vv[j])),
+                 make_uint4(o[0], o[1], o[2], o[3]));
+      }
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Q4 of fp8 pages (1-byte engines, B200KV_DTYPE_E4M3 / B200KV_DTYPE_E5M2; spec: tests/fp8_cache_oracle.py).  The
+// record is the one above, bf16 scales included.  A 16-byte vector holds 16 codes, so a group of 32 elements is a
+// pair of lanes (one shuffle); each vector writes 8 code bytes and the even lane of the pair writes the scale.
+// Codes decode exactly to fp32 through f16 (cvt.rn.f16x2.e4m3x2 / e5m2x2).  The group absmax is taken on the 7
+// magnitude bits: their integer order is magnitude order, finite codes below inf (e5m2) below NaN.  The store then
+// quantises like kv_q4_store_kernel; the load computes q * s exactly in fp32 and encodes it once with
+// cvt.rn.satfinite to the cache's type.  vLLM's k_scale / v_scale multiply the code's value on both sides of the
+// cache, so they cancel and neither kernel needs them.  Units, runs and addressing (q4_src_addr, NHD and HND) are
+// those of the 16-bit kernels: row_bytes is D here.
+// ---------------------------------------------------------------------------------------------
+template <__nv_fp8_interpretation_t FT>
+__device__ __forceinline__ float2 fp8x2_to_f32(uint32_t two_codes) {
+  const __half2_raw h = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(two_codes & 0xffffu), FT);
+  return __half22float2(*reinterpret_cast<const __half2*>(&h));
+}
+
+template <__nv_fp8_interpretation_t FT>
+__global__ void __launch_bounds__(256) kv_q4_store_fp8_kernel(const KernelArgs p) {
+  const uint32_t vpt = (p.n_heads * p.row_bytes) >> 4;      // vectors per token (even: D % 32 == 0)
+  const uint32_t vpt_shift = (vpt & (vpt - 1)) == 0 ? 31u - __clz(vpt) : 0xffffffffu;
+  const uint32_t codes_bytes = vpt * 8;
+  const bool st8 = (p.chunk.token_bytes & 7u) == 0;         // records 8-byte aligned (else 4: H*D % 64 == 0)
+  for (uint32_t ui = blockIdx.x; ui < p.total_units; ui += gridDim.x) {
+    const uint32_t plane = p.plane_begin + ui % p.n_planes;
+    const Run run = p.runs[ui / p.n_planes];
+    const ChunkPos cp = chunk_pos(p.chunk, static_cast<uint32_t>(run.b));
+    const uint32_t t0 = cp.t;
+    uint8_t* slab =
+        reinterpret_cast<uint8_t*>(__ldg(p.chunk.chunk_addrs + cp.c) + static_cast<uint64_t>(plane) * p.chunk.slab_bytes);
+    const uint32_t nvec = static_cast<uint32_t>(run.n) * vpt;
+    for (uint32_t base = 0; base < nvec; base += 256 * kQ4Unroll) {   // uniform trip count: every lane shuffles
+      uint4 x[kQ4Unroll];
+      uint32_t tt[kQ4Unroll], vv[kQ4Unroll];
+      bool ok[kQ4Unroll];
+#pragma unroll
+      for (int j = 0; j < kQ4Unroll; ++j) {                 // all loads first: kQ4Unroll x 16 B in flight per thread
+        const uint32_t idx = base + j * 256 + threadIdx.x;   // 256 and vpt are even: pairs stay whole
+        ok[j] = idx < nvec;
+        tt[j] = vv[j] = 0;
+        if (ok[j]) q4_split(idx, vpt, vpt_shift, &tt[j], &vv[j]);
+        x[j] = ok[j] ? ld_nc_v4(reinterpret_cast<const void*>(q4_src_addr(p, plane, static_cast<uint32_t>(run.a) + tt[j], vv[j])))
+                     : make_uint4(0, 0, 0, 0);
+      }
+#pragma unroll
+      for (int j = 0; j < kQ4Unroll; ++j) {
+        const uint32_t w[4] = {x[j].x, x[j].y, x[j].z, x[j].w};
+        uint32_t acc = __vmaxu4(__vmaxu4(w[0] & 0x7f7f7f7fu, w[1] & 0x7f7f7f7fu), __vmaxu4(w[2] & 0x7f7f7f7fu, w[3] & 0x7f7f7f7fu));
+        acc = max(max(acc & 0xffu, (acc >> 8) & 0xffu), max((acc >> 16) & 0xffu, acc >> 24));
+        const uint32_t m = max(acc, __shfl_xor_sync(0xffffffffu, acc, 1));
+        const float amax = fp8x2_to_f32<FT>(m).x;
+        const __nv_bfloat16 sb = m ? __float2bfloat16_rn(__fdiv_rn(amax, 7.0f)) : __float2bfloat16_rn(1.0f);
+        const float inv = __fdiv_rn(1.0f, __bfloat162float(sb));
+        // rint(x * inv) by fma(x, inv, 1.5 * 2^23), as in kv_q4_store_kernel
+        uint32_t packed[2] = {0u, 0u};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const float2 a = fp8x2_to_f32<FT>(w[i]), b = fp8x2_to_f32<FT>(w[i] >> 16);
+          const uint32_t q0 = __float_as_uint(__fmaf_rn(a.x, inv, 12582912.0f)) & 0xFu;
+          const uint32_t q1 = __float_as_uint(__fmaf_rn(a.y, inv, 12582912.0f)) & 0xFu;
+          const uint32_t q2 = __float_as_uint(__fmaf_rn(b.x, inv, 12582912.0f)) & 0xFu;
+          const uint32_t q3 = __float_as_uint(__fmaf_rn(b.y, inv, 12582912.0f)) & 0xFu;
+          packed[i >> 1] |= (q0 | (q1 << 4) | (q2 << 8) | (q3 << 12)) << (16 * (i & 1));
+        }
+        if (!ok[j]) continue;
+        uint8_t* rec = slab + static_cast<uint64_t>(t0 + tt[j]) * p.chunk.token_bytes;
+        uint8_t* codes = rec + static_cast<size_t>(vv[j]) * 8;
+        if (st8) {
+          *reinterpret_cast<uint2*>(codes) = make_uint2(packed[0], packed[1]);
+        } else {
+          reinterpret_cast<uint32_t*>(codes)[0] = packed[0];
+          reinterpret_cast<uint32_t*>(codes)[1] = packed[1];
+        }
+        if ((vv[j] & 1u) == 0) *reinterpret_cast<__nv_bfloat16*>(rec + codes_bytes + static_cast<size_t>(vv[j] >> 1) * 2) = sb;
+      }
+    }
+  }
+}
+
+template <__nv_fp8_interpretation_t FT>
+__global__ void __launch_bounds__(256) kv_q4_load_fp8_kernel(const KernelArgs p) {
+  const uint32_t vpt = (p.n_heads * p.row_bytes) >> 4;
+  const uint32_t vpt_shift = (vpt & (vpt - 1)) == 0 ? 31u - __clz(vpt) : 0xffffffffu;
+  const uint32_t codes_bytes = vpt * 8;
+  const bool ld8 = (p.chunk.token_bytes & 7u) == 0;
+  for (uint32_t ui = blockIdx.x; ui < p.total_units; ui += gridDim.x) {
+    const uint32_t plane = p.plane_begin + ui % p.n_planes;
+    const Run run = p.runs[ui / p.n_planes];
+    const ChunkPos cp = chunk_pos(p.chunk, static_cast<uint32_t>(run.b));
+    const uint32_t t0 = cp.t;
+    const uint8_t* slab = reinterpret_cast<const uint8_t*>(__ldg(p.chunk.chunk_addrs + cp.c) +
+                                                           static_cast<uint64_t>(plane) * p.chunk.slab_bytes);
+    const uint32_t nvec = static_cast<uint32_t>(run.n) * vpt;
+    for (uint32_t base = threadIdx.x; base < nvec; base += 256 * kQ4Unroll) {
+      uint2 packed[kQ4Unroll];
+      uint32_t tt[kQ4Unroll], vv[kQ4Unroll];
+      uint16_t sbits[kQ4Unroll];
+#pragma unroll
+      for (int j = 0; j < kQ4Unroll; ++j) {                 // all loads first
+        const uint32_t idx = base + j * 256;
+        packed[j] = make_uint2(0, 0);
+        sbits[j] = 0;
+        tt[j] = vv[j] = 0;
+        if (idx < nvec) {
+          q4_split(idx, vpt, vpt_shift, &tt[j], &vv[j]);
+          const uint8_t* rec = slab + static_cast<uint64_t>(t0 + tt[j]) * p.chunk.token_bytes;
+          const uint8_t* codes = rec + static_cast<size_t>(vv[j]) * 8;
+          if (ld8) {
+            packed[j] = __ldg(reinterpret_cast<const uint2*>(codes));
+          } else {
+            packed[j].x = __ldg(reinterpret_cast<const uint32_t*>(codes));
+            packed[j].y = __ldg(reinterpret_cast<const uint32_t*>(codes) + 1);
+          }
+          sbits[j] = __ldg(reinterpret_cast<const uint16_t*>(rec + codes_bytes + static_cast<size_t>(vv[j] >> 1) * 2));
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < kQ4Unroll; ++j) {
+        if (base + j * 256 >= nvec) continue;
+        const float s = __uint_as_float(static_cast<uint32_t>(sbits[j]) << 16);
+        const uint32_t pw[2] = {packed[j].x, packed[j].y};
+        uint32_t o[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int b = static_cast<int>((pw[i >> 1] >> (16 * (i & 1))) & 0xffffu);
+          const int q0 = ((b & 0xF) ^ 8) - 8, q1 = (((b >> 4) & 0xF) ^ 8) - 8;   // sign-extend the nibbles
+          const int q2 = (((b >> 8) & 0xF) ^ 8) - 8, q3 = ((b >> 12) ^ 8) - 8;
+          const uint32_t lo = __nv_cvt_float2_to_fp8x2(make_float2(static_cast<float>(q0) * s, static_cast<float>(q1) * s),
+                                                       __NV_SATFINITE, FT);
+          const uint32_t hi = __nv_cvt_float2_to_fp8x2(make_float2(static_cast<float>(q2) * s, static_cast<float>(q3) * s),
+                                                       __NV_SATFINITE, FT);
+          o[i] = lo | (hi << 16);
         }
         st_na_v4(reinterpret_cast<void*>(q4_src_addr(p, plane, static_cast<uint32_t>(run.a) + tt[j], vv[j])),
                  make_uint4(o[0], o[1], o[2], o[3]));
